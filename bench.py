@@ -19,9 +19,9 @@ e2e   : the weak metric with feature maps in pinned HOST memory (H2D inside the 
         back to the host.
 parity: every run checks its own output: two of the timed layer problems are re-solved by the CPU oracle on the
         same arrays (mask, alpha-probe sequence, weights, bias).
-Inputs per step (~18 GB of feature maps per network) are far larger than the 126 MB L2, so no L2
-flush is needed between timed iterations of the step; the stand-alone kernel timings for the
-rooflines flush L2 explicitly.
+Inputs per step (~18 GB of feature maps per network) are far larger than the 50 MB L2 of an H100, so no
+L2 flush is needed between timed iterations of the step; the stand-alone kernel timings for the
+rooflines flush L2 explicitly.  --dump-outputs DIR: the last timed step's outputs as .npy (seeded inputs).
 """
 import argparse
 import json
@@ -57,7 +57,7 @@ def parse():
     ap.add_argument("--impl", default="cpb200", choices=["cpb200", "reference"])
     ap.add_argument("--streams", type=int, default=13)
     ap.add_argument("--gram", default="tc", choices=["tc", "fp64"],
-                    help="arithmetic of the big Gram products: tc = tcgen05 3xTF32 (default), fp64 = DFMA")
+                    help="arithmetic of the big Gram products: tc = split-fp16 wgmma (default), fp64 = DFMA")
     ap.add_argument("--layout", default="nhwc", choices=["nhwc", "nchw"],
                     help="HBM layout of the bottom blobs for the device-resident arm (nhwc: TMA gather; the host copies of "
                          "the e2e arm keep the reference's NCHW blob order)")
@@ -66,10 +66,17 @@ def parse():
     ap.add_argument("--no-parity", action="store_true")
     ap.add_argument("--no-strong", action="store_true", help="N > 1: skip the strong-scaling leg")
     ap.add_argument("--layers", default="", help="comma list of layer names (debug); default: all of the workload")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the outputs of the last timed step as DIR/<layer>_<what>.npy (float32/float64)")
     ap.add_argument("--workload", default="vgg16", choices=["vgg16", "resnet50", "sweep"],
                     help="vgg16 = BASELINE configs[1] (13 conv layers); resnet50 = configs[3] (48 bottleneck problems); "
                          "sweep = configs[4] (Gram roofline and LASSO data-form kernel against N)")
-    return ap.parse_args()
+    args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "cpb200" or args.workload == "sweep"):
+        ap.error("--dump-outputs writes the outputs of the GPU arm of the vgg16 / resnet50 workloads")
+    if args.dump_outputs and args.steps < 1:
+        ap.error("--dump-outputs needs at least one timed step")
+    return args
 
 
 def config_dict(args, base, world):
@@ -288,20 +295,12 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(sm)}
 
 
-def ncu_traffic():
-    """DRAM bytes per launch of the dominant kernels from the committed ncu --set full captures (profiles/)."""
-    p = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if os.path.exists(p):
-        return json.load(open(p))
-    return {}
-
-
 def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
         return d, "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0}, "fallback"
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data sheet"
 
 
 def library_peaks(torch, dev):
@@ -377,6 +376,27 @@ def parity_check(shapes, datas, results, names):
     out["pass"] = bool(out["layers_checked"] and out["mask_equal"] and out["probes_equal"] and
                        out["rel_W_max"] <= 1e-4 and out["rel_b_max"] <= 1e-4)
     return out
+
+
+DUMP_SAMPLE = 1 << 18  # weights larger than this are stored as a fixed sample (keeps a dump of the stack near 30 MB)
+
+
+def dump_outputs(out_dir, shapes, results, prefixes):
+    """What the timed path returned in its last step: per layer the kept-channel mask, the reconstructed weights
+    (float64; a fixed seeded sample of DUMP_SAMPLE entries when larger), the bias and the chosen alpha."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    for s, r, pre in zip(shapes, results, prefixes):
+        W = (r.W.cpu() if r.W.is_cuda else r.W).numpy().astype(np.float64).reshape(-1)
+        sampled = W.size > DUMP_SAMPLE
+        if sampled:
+            W = W[np.sort(np.random.RandomState(0).choice(W.size, DUMP_SAMPLE, replace=False))]
+        arrays = {"mask": np.asarray(r.idxs, dtype=np.float32), "W_sample" if sampled else "W": W,
+                  "b": (r.b.cpu() if r.b.is_cuda else r.b).numpy().astype(np.float64).reshape(-1),
+                  "alpha": np.array([float(r.alpha)], dtype=np.float64)}
+        for what, a in arrays.items():
+            np.save(os.path.join(out_dir, "%s%s_%s.npy" % (pre, s.name, what)), a)
 
 
 # ------------------------------------------------------------------------------ GPU arm
@@ -481,6 +501,9 @@ def run_gpu(args):
     clocks = sampler.stop() if rank == 0 else None
     total_layers = len(shapes) * args.steps
     value = total_layers / (ms / 1e3)
+    if args.dump_outputs:  # with several networks in the pool (N > 1 GPUs) each rank writes its own, prefixed netK_
+        dump_outputs(args.dump_outputs, my_shapes, res,
+                     ["net%d_" % (i // len(base)) if world > 1 else "" for i in mine])
 
     parity = None
     if rank == 0 and not args.no_parity:
@@ -549,18 +572,16 @@ def run_gpu(args):
     if rank == 0:
         peaks, which = measured_peaks()
         peaks_lib = library_peaks(torch, dev)
-        traffic = ncu_traffic()
         s = max(base, key=lambda q: q.K)
         names = [shapes[i].name for i in mine]
         d = datas[names.index(s.name)] if s.name in names else cpb200.synth.make_problem_device(s, 5, eng, layout=args.layout)
         lay = d.get("layout", "nchw")
         X = eng.patch_gather(d["fmap"], d["randx"], d["randy"], s.B, s.P, s.k, s.pad, s.stride, relu=True, layout=lay)
         fp64_mode = eng.gram_mode == cpb200.engine.GRAM_FP64
-        gen1 = os.environ.get("CPB200_GRAM_TC", "") == "1"
         kern_ms = []
         t_ms = timed_alone(torch, dev, lambda: eng.gram(X, d["feats"], y_bias=d["b2"], want_sums=False))
-        if not fp64_mode and not gen1:
-            # second pass with CUDA events around the tcgen05 GEMM launch (on its stream), read after each call
+        if not fp64_mode:
+            # second pass with CUDA events around the tensor-core GEMM launch (on its stream), read after each call
             eng.gram_profile(True)
 
             def one_gram():
@@ -575,37 +596,29 @@ def run_gpu(args):
             kernel, k_ms = "cp_gram (fp64 products)", t_ms
             peak, peak_note = peaks_lib["fp64_tflops"], "cuBLAS FP64 GEMM 4096^3 measured in this run"
             extra = {}
-        elif gen1:
-            kernel, k_ms = "cp_gram, first-generation gram_tc_kernel (3xTF32) + its passes", t_ms
-            peak, peak_note = peaks_lib["tf32_tflops"], "cuBLAS TF32 GEMM 8192^3 measured in this run; 3 MMAs per product: ceiling 1/3"
-            extra = {}
         else:
-            # the dominant kernel of the call, timed alone: gram_tc2_pair_kernel (kind::f16 tcgen05, three products of
-            # the split-fp16 operands per algorithmic product -> ceiling = 1/3 of the dense 16-bit rate)
+            # the dominant kernel of the call, timed alone: gram_tc2_kernel (fp16 wgmma, three products of the
+            # split-fp16 operands per algorithmic product -> ceiling = 1/3 of the dense 16-bit rate)
             k_ms = sum(kern_ms[2:]) / max(1, len(kern_ms[2:]))
-            kernel = "gram_tc2_pair_kernel (tcgen05 kind::f16, cta_group::2, 256x256 tiles; 3 MMAs per product)"
+            kernel = "gram_tc2_kernel (wgmma m64n128k16 f16, 128x128 tiles; 3 MMAs per product)"
             peak = peaks["bf16_tflops"]
-            peak_note = "dense bf16 burst of MEASURED_PEAKS.json (%s); split-precision scheme issues 3 MMAs per " \
-                        "algorithmic product: ceiling 1/3" % which
+            peak_note = "dense bf16 rate (%s); split-precision scheme issues 3 MMAs per " \
+                        "algorithmic product: ceiling 1/3" % ("MEASURED_PEAKS.json" if which == "measured" else which)
             extra = {"issued_tflops": 3.0 * flops / (k_ms / 1e3) / 1e12, "frac_issued": 3.0 * flops / (k_ms / 1e3) / 1e12 / peak,
                      "call": {"what": "whole cp_gram call (statistics passes, operand preparation, GEMM, fp64 reduction "
                                       "of the splits, lower triangle)", "ms": t_ms, "achieved": call_tflops,
                               "frac": call_tflops / peak},
                      "cublas_tf32_tflops": peaks_lib["tf32_tflops"]}
         achieved = flops / (k_ms / 1e3) / 1e12
-        tr = traffic.get("gram_tc2_pair_kernel" if not gen1 else "gram_tc_kernel") if not fp64_mode else None
         roof = {"kernel": "%s on %s: N=%d K=%d n=%d (X'X upper tiles + X'Y)" % (kernel, s.name, s.N, s.K, s.n),
                 "bound": "tensor" if not fp64_mode else "fp64-pipe",
                 "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
-                "traffic": tr["bytes"] if tr and s.name == "conv4_2" and s.N == 5000 else None,
-                "traffic_source": tr["source"] if tr else None,
                 "ms": k_ms, "algorithmic_flops": flops, "peak_source": peak_note,
-                "mode": "fp64" if fp64_mode else ("3xtf32" if gen1 else "3xfp16-split")}
+                "mode": "fp64" if fp64_mode else "3xfp16-split"}
         roof.update(extra)
         t_g = timed_alone(torch, dev, lambda: eng.patch_gather(d["fmap"], d["randx"], d["randy"], s.B, s.P, s.k, s.pad,
                                                                s.stride, relu=True, out=X, layout=lay))
         gbytes = 8.0 * s.N * s.K  # SURVEY.md 8(d): unique patch elements read + X written
-        trg = traffic.get("patch_gather_nhwc_tma" if lay == "nhwc" else "patch_gather")
         # the other layout, for the record (same values, same X)
         fm_other = cpb200.synth.fmap_nchw(d).contiguous() if lay == "nhwc" else d["fmap"].permute(0, 2, 3, 1).contiguous()
         other = "nchw" if lay == "nhwc" else "nhwc"
@@ -619,8 +632,9 @@ def run_gpu(args):
                   "other_layout": {"layout": other, "ms": t_o, "GB/s": gbytes / (t_o / 1e3) / 1e9, "X_bit_identical": same_X},
                   "bound": "hbm", "achieved": gbytes / (t_g / 1e3) / 1e9, "peak": peaks["hbm_gbs"], "unit": "GB/s",
                   "frac": gbytes / (t_g / 1e3) / 1e9 / peaks["hbm_gbs"],
-                  "traffic": trg["bytes"] if trg else None, "traffic_source": trg["source"] if trg else None,
-                  "ms": t_g, "algorithmic_bytes": gbytes, "peak_source": "%s copy bandwidth (MEASURED_PEAKS.json)" % which}
+                  "ms": t_g, "algorithmic_bytes": gbytes,
+                  "peak_source": ("copy bandwidth (MEASURED_PEAKS.json)" if which == "measured"
+                                  else "HBM3 bandwidth of the %s" % which)}
 
     cpu = None
     if rank == 0 and world == 1 and not args.no_cpu:

@@ -1,4 +1,4 @@
-"""cpb200 -- B200-native channel-pruning solver (hot path of ethanhe42/channel-pruning).
+"""cpb200 -- H100-native channel-pruning solver (hot path of ethanhe42/channel-pruning).
 
 The directory name carries a hyphen (it mirrors the reference repo's name), so import it as
 ``import cpb200`` (alias module at the repo root) or ``importlib.import_module
@@ -13,7 +13,7 @@ The directory name carries a hyphen (it mirrors the reference repo's name), so i
 import os as _os
 
 # One stream per layer problem (13+ in flight) needs as many hardware work queues: with the default 8 the
-# streams alias and a stream waiting on its transfer stalls unrelated layers (profiles/r1c_summary.md).
+# streams alias and a stream waiting on its transfer stalls unrelated layers.
 # Read by the driver when the CUDA context is created, so it must be set before the first CUDA call.
 _os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "32")
 

@@ -47,7 +47,7 @@ def load():
         if not os.path.exists(LIBRARY):
             raise ImportError(
                 "libcpb200.so not found at %s -- build it with `python -c 'import __graft_entry__ as g; "
-                "g.build()'` (nvcc, sm_100a).  There is no CPU fallback." % LIBRARY)
+                "g.build()'` (nvcc, sm_90a).  There is no CPU fallback." % LIBRARY)
         ffi = cffi.FFI()
         ffi.cdef(_cdef_text())
         _lib = ffi.dlopen(LIBRARY)

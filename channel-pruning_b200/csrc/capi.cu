@@ -17,8 +17,8 @@ extern "C" int cp_create(cp_handle_t *out, int device) {
     CP_REQUIRE(device >= 0 && device < ndev, "cp_create: device %d out of range (%d visible)", device, ndev);
     cudaDeviceProp prop;
     CP_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10)
-        CP_FAIL(CP_ERR_CUDA, "cp_create: device %d is sm_%d%d; libcpb200 is built for sm_100a only", device,
+    if (prop.major != 9 || prop.minor != 0)
+        CP_FAIL(CP_ERR_CUDA, "cp_create: device %d is sm_%d%d; libcpb200 is built for sm_90a only", device,
                 prop.major, prop.minor);
     cp_handle_s *h = new cp_handle_s();
     h->device = device;

@@ -227,7 +227,7 @@ int cp_patch_gather_tma(cp_handle_t h, const float *fmap, int nbatch, int B, int
     per_sm = per_sm < 1 ? 1 : (per_sm > 4 ? 4 : per_sm);
     static const int env_per_sm = [] { const char *e = getenv("CPB200_GATHER_CTAS_PER_SM"); return e ? atoi(e) : 0; }();
     static const int env_stages = [] { const char *e = getenv("CPB200_GATHER_STAGES"); return e ? atoi(e) : 0; }();
-    if (env_per_sm > 0 && env_per_sm < per_sm) per_sm = env_per_sm;  // tuning knobs (profiles/r2_run9.sh)
+    if (env_per_sm > 0 && env_per_sm < per_sm) per_sm = env_per_sm;  // tuning knobs
     int nstage = (int)((budget / per_sm - 1024 - GT_OUT * out_b) / row);
     if (nstage > 6) nstage = 6;
     if (env_stages >= 2 && env_stages < nstage) nstage = env_stages;

@@ -45,7 +45,7 @@ struct Args {
     int tile_mode;
     int a_vec, b_vec;       // 16-byte vector loads allowed (alignment checked by the host)
     int max_ctas;           // > 0: at most that many CTAs walk the tiles (leaves SMs free for latency-bound kernels of
-                            // other streams: a resident 128 x 128 x 256 tile holds its SM for ~60 us)
+                            // other streams: a resident 128 x 128 x 256 tile holds its SM for a long time)
 };
 
 template <typename T>

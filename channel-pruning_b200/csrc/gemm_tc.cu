@@ -7,15 +7,14 @@
 // The reference solves its least squares in float64 LAPACK (lib/decompose.py:665-666).  In the tensor-core mode the
 // normal equations already carry the 4e-7 of the split-precision Gram (gram_tc2.cu) and every solve is followed by a
 // refinement step from the data; the FP64 pipe, not accuracy, is what bounds the 13-layer step (~7.6e11 fp64 flop).
-// This kernel takes the GEMM-shaped bulk of those flops to tcgen05:
+// This kernel takes the GEMM-shaped bulk of those flops to wgmma:
 //
 //   prep   row scale 2^e (power of two, exact: max|row| * 2^e in [2^9, 2^10)), v = fl32(x 2^e) = hi + lo with
 //          hi = fp16_rn(v), lo = fp16_rn(v - hi) -- 22 mantissa bits of every operand entry, K-major rows, zero padded
-//   gemm   hi'hi + hi'lo + lo'hi on kind::f16 tcgen05.mma, CTA pairs (cta_group::2, 256 x 256 tiles), the TMA / MMA
-//          pipeline of gram_tc2_pair_kernel; fp32 accumulation in tensor memory, runs of 128 reduction elements
-//          alternating between the two accumulators (each takes at most half of the reduction)
-//   epilogue  C = beta C + alpha 2^-(eA_i + eB_j) acc, read-modify-write in fp64 straight from the drain warps
-//             (thread = one row x 128 columns: 32-byte sectors fully used)
+//   gemm   hi'hi + hi'lo + lo'hi on wgmma (128 x 128 tiles), the TMA -> wgmma pipeline of tc_common.cuh: fp32
+//          accumulation in registers in runs of 64 reduction elements, added with round-to-nearest
+//   epilogue  C = beta C + alpha 2^-(eA_i + eB_j) acc, read-modify-write in fp64 straight from the accumulator
+//             fragments (pairs of adjacent columns: 16-byte accesses)
 //
 // Error per product sum: <= ~2.4e-7 * sum_r |a||b| (the dropped lo'lo term and the fp32 accumulation), i.e. relative to
 // sqrt(C_ii C_jj) for the symmetric updates of a Cholesky factorisation, summed over all updates (sum_k L_ik^2 = G_ii).
@@ -31,21 +30,6 @@ namespace {
 
 using namespace cptc;
 
-constexpr int NDRAIN_WARPS = 8;
-constexpr int NTHREADS = 32 * (NDRAIN_WARPS + 2);
-constexpr int W_TMA = NDRAIN_WARPS, W_MMA = NDRAIN_WARPS + 1;
-constexpr int T_TMA = 32 * W_TMA;
-constexpr int SUB_STAGES = 2;                      // stages per accumulator run (128 reduction elements)
-constexpr int PS_TILE = 128 * 128;                 // bytes of one 128-row operand tile (hi or lo)
-constexpr int PS_STAGE_BYTES = 4 * PS_TILE;        // A hi, A lo, B-half hi, B-half lo
-constexpr int PS_STAGES = 2;                       // short reductions (R <= 1024): two stages leave room for the epilogue tiles
-constexpr int PS_OFF_BAR = PS_STAGES * PS_STAGE_BYTES;
-constexpr int PS_NBAR = 2 * PS_STAGES + 2;
-constexpr int PS_OFF_TMEM = PS_OFF_BAR + PS_NBAR * 8;
-constexpr int EP_LD = 66;                          // floats per row of a drain warp's 32 x 64 transposition tile
-constexpr int PS_OFF_EPI = (PS_OFF_TMEM + 16 + 15) / 16 * 16;
-constexpr int PS_SMEM_BYTES = PS_OFF_EPI + NDRAIN_WARPS * 32 * EP_LD * 4 + 1024;
-
 struct GtParams {
     double *C;
     int64_t ldc;
@@ -53,7 +37,7 @@ struct GtParams {
     double alpha, beta;
     int M, Nn;
     int nst;       // stages = padded reduction / 64
-    int tm, tn;    // 256-row tiles of A / B
+    int tm, tn;    // 128-row tiles of A / B
     int lower;     // only tiles with ti >= tj
     int ntiles;
     int same;      // B operand rows are the first rows of the A operand (symmetric update): diagonal tiles share A and B
@@ -80,187 +64,46 @@ __device__ __forceinline__ GtItem gt_decode(const GtParams &P, int w) {
     return it;
 }
 
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NTHREADS, 1)
-gemm_tc_pair_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const GtParams P) {
+__global__ void __launch_bounds__(NTHREADS, 1)
+gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const GtParams P) {
     extern __shared__ unsigned char smem_dyn[];
     unsigned char *smem = (unsigned char *)(((uintptr_t)smem_dyn + 1023) & ~(uintptr_t)1023);
     const uint32_t sbase = smem_u32(smem);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const bool leader = rank == 0;
-    const int ncl = gridDim.x >> 1, cid = blockIdx.x >> 1;
-    const int nitems = P.ntiles;
-
-    auto bar = [&](int i) { return sbase + PS_OFF_BAR + 8 * i; };
-    constexpr int FULL = 0, EMPTY = PS_STAGES, ACC_FULL = 2 * PS_STAGES, ACC_EMPTY = 2 * PS_STAGES + 1;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(smem + PS_OFF_TMEM);
-
-    if (threadIdx.x == T_TMA) {
-        for (int s = 0; s < PS_STAGES; ++s) {
-            mbar_init(bar(FULL + s), 1);
-            mbar_init(bar(EMPTY + s), 1);
-        }
-        mbar_init(bar(ACC_FULL), 1);
-        mbar_init(bar(ACC_EMPTY), 2 * NDRAIN_WARPS);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == W_MMA) {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    cluster_sync_all();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
-
+    pipe_init(sbase);
+    uint32_t g = 0;
     if (warp == W_TMA) {
-        if (lane == 0) {
-            uint32_t g = 0;
-            for (int w = cid; w < nitems; w += ncl) {
+        if (lane == 0)
+            for (int w = blockIdx.x; w < P.ntiles; w += gridDim.x) {
                 const GtItem it = gt_decode(P, w);
-                const int rowA = it.ti * 256 + (int)rank * 128, rowB = it.tj * 256 + (int)rank * 128;
-                for (int st = 0; st < P.nst; ++st, ++g) {
-                    const int s = g % PS_STAGES;
-                    const uint32_t ph = (g / PS_STAGES) & 1;
-                    mbar_wait(bar(EMPTY + s), ph ^ 1);
-                    const uint32_t dst = sbase + s * PS_STAGE_BYTES;
-                    const uint32_t lbar = mapa_rank(bar(FULL + s), 0);
-                    const int r0 = st * KS;
-                    if (leader) mbar_arrive_expect_tx(bar(FULL + s), 2 * (it.diag ? 2 * PS_TILE : PS_STAGE_BYTES));
-                    if (!it.diag) {
-                        tma_load_2d_pair(dst, &mapA, lbar, r0, rowA);
-                        tma_load_2d_pair(dst + PS_TILE, &mapA, lbar, r0, P.rowsA + rowA);
-                    }
-                    tma_load_2d_pair(dst + 2 * PS_TILE, &mapB, lbar, r0, rowB);
-                    tma_load_2d_pair(dst + 3 * PS_TILE, &mapB, lbar, r0, P.rowsB + rowB);
-                }
+                pipe_produce(sbase, g, &mapA, &mapB, it.ti * TILE, P.rowsA, it.tj * TILE, P.rowsB, 0, P.nst, it.diag);
             }
-        }
-    } else if (warp == W_MMA) {
-        // One tile = nst stages in runs of SUB_STAGES; run r accumulates into tensor-memory accumulator (r & 1), so that
-        // no fp32 accumulator takes more than half of the reduction (the tensor core truncates when it adds); both are
-        // handed to the drain warps at the end of the tile.
-        if (leader && lane == 0) {
-            const uint32_t idesc = (1u << 4) | ((uint32_t)(256 >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-            uint32_t g = 0, nt = 0;
-            for (int w = cid; w < nitems; w += ncl, ++nt) {
-                const GtItem it = gt_decode(P, w);
-                mbar_wait(bar(ACC_EMPTY), (nt & 1) ^ 1);  // both accumulators drained
-                for (int st = 0; st < P.nst; ++st, ++g) {
-                    const int s = g % PS_STAGES;
-                    const uint32_t ph = (g / PS_STAGES) & 1;
-                    const int run = st / SUB_STAGES, kk = st % SUB_STAGES;
-                    mbar_wait(bar(FULL + s), ph);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const uint32_t stage = sbase + s * PS_STAGE_BYTES;
-                    const uint32_t b_hi = stage + 2 * PS_TILE, b_lo = stage + 3 * PS_TILE;
-                    const uint32_t a_hi = it.diag ? b_hi : stage, a_lo = it.diag ? b_lo : stage + PS_TILE;
-                    const uint32_t acc = tmem_base + (uint32_t)(run & 1) * 256;
-#pragma unroll
-                    for (int ks = 0; ks < KS / 16; ++ks) {
-                        const uint32_t off = ks * 32;
-                        const uint32_t first = (run < 2 && kk == 0 && ks == 0) ? 0u : 1u;
-                        umma_f16_ss_pair(acc, umma_desc_k_sw128(a_hi + off), umma_desc_k_sw128(b_hi + off), idesc, first);
-                        umma_f16_ss_pair(acc, umma_desc_k_sw128(a_hi + off), umma_desc_k_sw128(b_lo + off), idesc, 1u);
-                        umma_f16_ss_pair(acc, umma_desc_k_sw128(a_lo + off), umma_desc_k_sw128(b_hi + off), idesc, 1u);
-                    }
-                    umma_commit_pair(bar(EMPTY + s));
-                }
-                umma_commit_pair(bar(ACC_FULL));
-            }
-        }
-    } else {
-        // drain warps of both CTAs.  A warp owns 32 accumulator rows (its TMEM lane quadrant) x 128 columns; tcgen05.ld
-        // hands every lane ONE ROW, but a read-modify-write of C with one row per lane is 32 transactions per
-        // instruction (measured: 30 us per tile).  So the accumulators pass through a per-warp shared-memory tile and
-        // leave transposed: one instruction = one row x 64 columns = 512 contiguous bytes, 16 rows in flight per lane.
-        const int quad = warp & 3, half = warp >> 2;
-        const uint32_t lane_addr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(half * 128);
-        const bool two = P.nst > SUB_STAGES;  // the second accumulator holds the odd runs
-        const bool vec = ((reinterpret_cast<uintptr_t>(P.C) & 15) == 0) && ((P.ldc & 1) == 0);
-        float *tile = reinterpret_cast<float *>(smem + PS_OFF_EPI) + warp * 32 * EP_LD;
-        uint32_t nt = 0;
-        for (int w = cid; w < nitems; w += ncl, ++nt) {
-            const GtItem it = gt_decode(P, w);
-            const int ibase = it.ti * 256 + (int)rank * 128 + quad * 32;   // first row of this warp
-            const int jbase = it.tj * 256 + half * 128;                      // first column of this warp
-            // the drain warps idle while the operands load and the MMAs run: pull this warp's 32 x 128 block of C
-            // (32 KB) into L2 meanwhile, so that the read-modify-write below does not start from DRAM latency
-            if (P.beta != 0.0 && ibase + lane < P.M) {
-                const double *crow = P.C + (int64_t)(ibase + lane) * P.ldc + jbase;
-#pragma unroll
-                for (int q = 0; q < 8; ++q)
-                    if (jbase + q * 16 < P.Nn) asm volatile("prefetch.global.L2 [%0];" ::"l"(crow + q * 16));
-            }
-            mbar_wait(bar(ACC_FULL), nt & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-            for (int p = 0; p < 2; ++p) {
-                {
-                    uint32_t r0[32], r1[32];
-#pragma unroll
-                    for (int hh = 0; hh < 2; ++hh) {
-                        tmem_ld32(lane_addr + (uint32_t)(p * 64 + hh * 32), r0);
-                        if (two) tmem_ld32(lane_addr + 256 + (uint32_t)(p * 64 + hh * 32), r1);
-                        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                        for (int e = 0; e < 32; ++e)
-                            tile[lane * EP_LD + hh * 32 + e] =
-                                two ? __fadd_rn(__uint_as_float(r0[e]), __uint_as_float(r1[e])) : __uint_as_float(r0[e]);
-                    }
-                }
-                __syncwarp();
-                const int j = jbase + p * 64 + 2 * lane;  // this lane's two columns
-                if (j < P.Nn && ibase < P.M) {
-                    const bool pairok = vec && (j + 1 < P.Nn);
-                    const double sj0 = P.invB[j], sj1 = (j + 1 < P.Nn) ? P.invB[j + 1] : 0.0;
-#pragma unroll 1
-                    for (int rb = 0; rb < 32; rb += 16) {
-                        double2 cv[16];
-                        if (P.beta != 0.0) {
-#pragma unroll
-                            for (int q = 0; q < 16; ++q) {
-                                const int i = ibase + rb + q;
-                                cv[q] = make_double2(0.0, 0.0);
-                                if (i < P.M) {
-                                    const double *src = P.C + (int64_t)i * P.ldc + j;
-                                    if (pairok) cv[q] = *reinterpret_cast<const double2 *>(src);
-                                    else { cv[q].x = src[0]; if (j + 1 < P.Nn) cv[q].y = src[1]; }
-                                }
-                            }
-                        } else {
-#pragma unroll
-                            for (int q = 0; q < 16; ++q) cv[q] = make_double2(0.0, 0.0);
-                        }
-#pragma unroll
-                        for (int q = 0; q < 16; ++q) {
-                            const int i = ibase + rb + q;
-                            const float2 v = *reinterpret_cast<const float2 *>(tile + (rb + q) * EP_LD + 2 * lane);
-                            if (i < P.M) {
-                                const double ai = P.alpha * __ldg(P.invA + i);  // same address in every lane: one broadcast
-                                cv[q].x = P.beta * cv[q].x + ai * sj0 * (double)v.x;
-                                cv[q].y = P.beta * cv[q].y + ai * sj1 * (double)v.y;
-                                double *dst = P.C + (int64_t)i * P.ldc + j;
-                                if (pairok) *reinterpret_cast<double2 *>(dst) = cv[q];
-                                else { dst[0] = cv[q].x; if (j + 1 < P.Nn) dst[1] = cv[q].y; }
-                            }
-                        }
-                    }
-                }
-                __syncwarp();  // the tile is rewritten by the next pass
-            }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(mapa_rank(bar(ACC_EMPTY), 0));
-        }
+        return;
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    cluster_sync_all();
-    if (warp == W_MMA) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512));
+    const int wg = warp >> 2;
+    const bool vec = ((reinterpret_cast<uintptr_t>(P.C) & 15) == 0) && ((P.ldc & 1) == 0);
+    for (int w = blockIdx.x; w < P.ntiles; w += gridDim.x) {
+        const GtItem it = gt_decode(P, w);
+        float sum[FRAG];
+        pipe_consume(sbase, g, wg, P.nst, it.diag, sum);
+        const int ibase = it.ti * TILE + wg * 64, jbase = it.tj * TILE;
+#pragma unroll
+        for (int e = 0; e < FRAG; e += 2) {
+            const int i = ibase + frag_row(e), j = jbase + frag_col(e);  // this thread's columns j, j + 1
+            if (i >= P.M || j >= P.Nn) continue;
+            const bool two = j + 1 < P.Nn;
+            double *dst = P.C + (int64_t)i * P.ldc + j;
+            double2 cv = make_double2(0.0, 0.0);
+            if (P.beta != 0.0) {
+                if (vec && two) cv = *reinterpret_cast<const double2 *>(dst);
+                else { cv.x = dst[0]; if (two) cv.y = dst[1]; }
+            }
+            const double ai = P.alpha * __ldg(P.invA + i);
+            cv.x = P.beta * cv.x + ai * __ldg(P.invB + j) * (double)sum[e];
+            cv.y = P.beta * cv.y + ai * (two ? __ldg(P.invB + j + 1) : 0.0) * (double)sum[e + 1];
+            if (vec && two) *reinterpret_cast<double2 *>(dst) = cv;
+            else { dst[0] = cv.x; if (two) dst[1] = cv.y; }
+        }
     }
 }
 
@@ -365,13 +208,13 @@ bool cp_gemm_tc_enabled() {
 // are ordered, so a buffer is never rewritten under a kernel that still reads it)
 // b_nc: the B operand is stored reduction-major, b(nn, r) = B[r * ldb + nn]
 int cp_gemm_tc_f64(cp_handle_t h, int slot, const double *A, int64_t lda, const double *B, int64_t ldb, double *C, int64_t ldc,
-                   int M, int Nn, int R, double alpha, double beta, int lower, cudaStream_t stream, int max_clusters,
+                   int M, int Nn, int R, double alpha, double beta, int lower, cudaStream_t stream, int max_ctas,
                    int b_nc) {
     if (M <= 0 || Nn <= 0) return CP_OK;
     CP_REQUIRE(slot >= 0 && slot < 3 && R > 0, "cp_gemm_tc_f64: bad slot / R");
     const bool same = (!b_nc && A == B && lda == ldb && Nn <= M);
     const int Rp = cp_cdiv(R, KS) * KS;
-    const int rowsA = cp_cdiv(M, 256) * 256, rowsB = same ? rowsA : cp_cdiv(Nn, 256) * 256;
+    const int rowsA = cp_cdiv(M, TILE) * TILE, rowsB = same ? rowsA : cp_cdiv(Nn, TILE) * TILE;
     const size_t needA = 2 * (size_t)rowsA * Rp * sizeof(__half), needB = same ? 0 : 2 * (size_t)rowsB * Rp * sizeof(__half);
     const size_t need = cp_align_up(needA, 256) + cp_align_up(needB, 256) + cp_align_up((size_t)(rowsA + 2 * rowsB) * 8, 256);
     if (need > h->tcbuf_bytes[slot]) {
@@ -405,24 +248,24 @@ int cp_gemm_tc_f64(cp_handle_t h, int slot, const double *A, int64_t lda, const 
         CP_CHECK_LAUNCH();
     }
     CUtensorMap mapA, mapB;
-    int rc = make_map16(h, &mapA, opA, Rp, 2 * (int64_t)rowsA, 128);
+    int rc = make_map16(h, &mapA, opA, Rp, 2 * (int64_t)rowsA, TILE);
     if (rc) return rc;
-    rc = make_map16(h, &mapB, opB, Rp, 2 * (int64_t)rowsB, 128);
+    rc = make_map16(h, &mapB, opB, Rp, 2 * (int64_t)rowsB, TILE);
     if (rc) return rc;
     GtParams P{};
     P.C = C; P.ldc = ldc; P.invA = invA; P.invB = invB; P.alpha = alpha; P.beta = beta; P.M = M; P.Nn = Nn;
-    P.nst = Rp / KS; P.tm = cp_cdiv(M, 256); P.tn = cp_cdiv(Nn, 256); P.lower = lower ? 1 : 0;
+    P.nst = Rp / KS; P.tm = cp_cdiv(M, TILE); P.tn = cp_cdiv(Nn, TILE); P.lower = lower ? 1 : 0;
     P.ntiles = lower ? P.tn * P.tm - P.tn * (P.tn - 1) / 2 : P.tm * P.tn;
     P.same = same ? 1 : 0; P.rowsA = rowsA; P.rowsB = rowsB;
     static cp_per_device_flag configured;
     if (bool *done = configured.slot(); !*done) {
-        CP_CUDA(cudaFuncSetAttribute(gemm_tc_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PS_SMEM_BYTES));
+        CP_CUDA(cudaFuncSetAttribute(gemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
         *done = true;
     }
-    int ncl = h->num_sms / 2;
-    if (max_clusters > 0 && max_clusters < ncl) ncl = max_clusters;
-    if (P.ntiles < ncl) ncl = P.ntiles;
-    gemm_tc_pair_kernel<<<2 * ncl, NTHREADS, PS_SMEM_BYTES, stream>>>(mapA, mapB, P);
+    int grid = h->num_sms;
+    if (max_ctas > 0 && max_ctas < grid) grid = max_ctas;
+    if (P.ntiles < grid) grid = P.ntiles;
+    gemm_tc_kernel<<<grid, NTHREADS, SMEM_BYTES, stream>>>(mapA, mapB, P);
     CP_CHECK_LAUNCH();
     return CP_OK;
 }

@@ -6,7 +6,7 @@
 // CP_GRAM_FP64: fp32 inputs widened to fp64 in registers, DFMA accumulation
 // (cpgemm::gemm_kernel).  Every product of two fp32 values is exact in fp64, so the
 // only rounding is the fp64 accumulation -- the same arithmetic class as the
-// reference's float64 numpy path.  Small K does not fill 148 SMs with output tiles,
+// reference's float64 numpy path.  Small K does not fill the SMs with output tiles,
 // so the reduction (row) dimension is split across CTAs into fp64 partials that a
 // second kernel sums in a fixed order (deterministic, no atomics).
 #include <stdlib.h>
@@ -14,9 +14,6 @@
 #include "common.cuh"
 #include "gemm_f64.cuh"
 
-int cp_gram_tc(cp_handle_t h, const float *X, int64_t N, int K, int64_t ldx, const void *Yraw, int y_dtype, int n, int64_t ldy,
-               const float *y_bias, const int32_t *rows, int nrows, double *G, double *Bxy, double *sx,
-               double *sy, double *yy, cudaStream_t stream);
 
 int cp_gram_tc2(cp_handle_t h, const float *X, int64_t N, int K, int64_t ldx, const void *Yraw, int y_dtype, int n, int64_t ldy,
                 const float *y_bias, const int32_t *rows, int nrows, double *G, double *Bxy, double *sx,
@@ -179,10 +176,6 @@ extern "C" int cp_gram(cp_handle_t h, const float *X, int64_t N, int K, int64_t 
         return CP_OK;
     }
     if (mode == CP_GRAM_3XTF32) {  // falls back to the fp64 products when TMA alignment rules are not met
-        // generation 2 (split-fp16 operands prepared once, gram_tc2.cu) unless CPB200_GRAM_TC=1 asks for the
-        // first-generation 3xTF32 kernel (gram_tc.cu; kept for A/B measurements)
-        static const bool gen1 = [] { const char *e = getenv("CPB200_GRAM_TC"); return e && e[0] == '1'; }();
-        if (gen1) return cp_gram_tc(h, X, N, K, ldx, Yraw, y_dtype, n, ldy, y_bias, rows, nrows, G, Bxy, sx, sy, yy, stream);
         return cp_gram_tc2(h, X, N, K, ldx, Yraw, y_dtype, n, ldy, y_bias, rows, nrows, G, Bxy, sx, sy, yy, stream);
     }
     return cp_gram_fp64_products(h, X, N, K, ldx, Yraw, y_dtype, n, ldy, y_bias, rows, nrows, G, Bxy, sx, sy, yy, stream);

@@ -1,37 +1,26 @@
-// cp_gram, tensor-core mode (CP_GRAM_3XTF32 in the header), second generation: split-fp16 operands prepared once,
-// a persistent TMA -> tcgen05 pipeline with no conversion work on the critical path.
+// cp_gram, tensor-core mode (CP_GRAM_3XTF32 in the header): split-fp16 operands prepared once, a persistent
+// TMA -> wgmma pipeline with no conversion work on the critical path.
 //
 //   G = X'X (K x K),  Bxy = X'(Y - b) (K x n)      X: N x K fp32 row-major, N ~ 5e3..1e5, K = c*k*k
 //
 // The reference does this arithmetic in float64 on the CPU (numpy matmul / LAPACK inside LinearRegression.fit,
-// lib/decompose.py:665-666, and the LASSO design products lib/decompose.py:428-457).  tcgen05 has no fp32/fp64
-// MMA; the first-generation kernel (gram_tc.cu) used three kind::tf32 products of a hi/lo split made by converter
-// warps inside the GEMM -- 46 % tensor-pipe utilisation, bound by the per-k-block hand-shake of those warps
-// (profiles/r1c_summary.md).  This version removes them:
+// lib/decompose.py:665-666, and the LASSO design products lib/decompose.py:428-457).  The tensor cores have no fp64
+// MMA at this rate, so the products are taken in three fp16 MMAs of a 22-bit hi/lo split:
 //
 //   prep   xs = fl32(x - s_col)             s = fp32 column mean (removes the rank-one mean component)
 //          v  = xs * 2^e_col                power-of-two column scale (exact): max|v| in [2^9, 2^10)
 //          v  = hi + lo                     hi = fp16_rn(v), lo = fp16_rn(v - hi): 22 mantissa bits kept -- the
-//                                           same split precision as tf32 (10 explicit bits each), but kind::f16
-//                                           runs at twice the tf32 rate and the operands are half as wide
+//                                           same split precision as tf32 (10 explicit bits each), but fp16 MMAs
+//                                           run at twice the tf32 rate and the operands are half as wide
 //          written TRANSPOSED (operand row = column of X, reduction index contiguous, zero padded) so that the
 //          GEMM reads plain K-major SWIZZLE_128B tiles with TMA; the same pass produces the fp64 column sums
 //          and sums of squares of xs (fixed summation order)
-//   gemm   P += hi'hi + hi'lo + lo'hi       three kind::f16 MMAs (128 x 256 x 16) per k-step, fp32 accumulation
-//          in TMEM, both operands from shared memory; the tensor core truncates when it adds into its fp32
-//          accumulator, so an accumulator takes 128 rows (24 additions), then the drain warps add it into fp32
-//          registers with round-to-nearest while the MMAs continue on the second accumulator
+//   gemm   P += hi'hi + hi'lo + lo'hi       three wgmma chains (m64n128k16) per k-step, fp32 accumulation in
+//          registers in runs of 64 rows, each run added into fp32 register sums with round-to-nearest
+//          (tc_common.cuh)
 //   reduce fp64 sum of the row splits, exact rescale by 2^-(e_i + e_j), shift undone exactly
 //          (G = P + s T' + T s' + N s s',  T = column sums of xs in fp64), diagonal from the fp64 squares,
 //          lower triangle written in the same pass.
-//
-// GEMM anatomy: persistent grid (one CTA per SM), static round-robin over (output tile, row split) items.
-//   warp 8   TMA producer: per 64-row stage four boxes (A hi/lo 64 x 128, B hi/lo 64 x 256; diagonal tiles take
-//            the A operand out of the B tile), 2 stages of 96 KB
-//   warp 9   TMEM allocator + single-thread MMA issuer; tcgen05.commit frees the stage / publishes the accumulator
-//   warps 0-7  drain: thread = accumulator row x 128 columns, tcgen05.ld, fp32 adds, one fp32 partial tile per item
-// Bound: L2 -> SM operand traffic (96 KB per 1536 tensor-pipe cycles = 62 B/clk/SM against ~42 B/clk/SM of L2
-// slice throughput), then the tensor pipe.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <stdlib.h>
@@ -49,66 +38,49 @@ namespace {
 
 using namespace cptc;
 
-constexpr int TM = 128, TN = 256;  // output tile (rows of A x rows of B), reduction rows per stage
-constexpr int A_TILE = TM * 128;            // bytes of one A operand tile (hi or lo): 128 rows x 128 B
-constexpr int B_TILE = TN * 128;
-constexpr int STAGE_BYTES = 2 * A_TILE + 2 * B_TILE;  // 96 KB
-constexpr int STAGES = 2;
-constexpr int SUB_STAGES = 2;               // stages per accumulator run (128 rows)
-constexpr int NDRAIN_WARPS = 8;
-constexpr int NTHREADS = 32 * (NDRAIN_WARPS + 2);
-constexpr int W_TMA = NDRAIN_WARPS, W_MMA = NDRAIN_WARPS + 1;  // single-thread roles on the highest warp ids
-constexpr int T_TMA = 32 * W_TMA;
-constexpr int OFF_BAR = STAGES * STAGE_BYTES;
-constexpr int NBAR = 2 * STAGES + 4;
-constexpr int OFF_TMEM = OFF_BAR + NBAR * 8;
-constexpr int SMEM_BYTES = OFF_TMEM + 16 + 1024;  // + alignment slack
+constexpr int TN = TILE;                    // output tile: 128 rows of G (or of X'Y) x 128 columns
 constexpr int RS = 32;                      // row splits of the statistics passes (partials combined in fixed order)
 constexpr int PT = 64;                      // prep tile: 64 rows x 64 columns
 
 struct Tc2Params {
-    float *partial;      // [nsplit][ntiles][128][256]
+    float *partial;      // [nsplit][ntiles][128][128]
     int64_t Np;          // padded row count (multiple of 64) = inner extent of the operand matrix
-    int rows_per_split;  // multiple of 128
+    int rows_per_split;  // multiple of 64
     int nsplit;
-    int tiles_sym;       // number of 128 x 256 tiles covering the upper triangle of G (0 when G is not requested)
-    int tk;              // ceil(K / 128): A tiles
-    int tjx;             // ceil(K / 256): B tiles inside X
-    int tjy0;            // first B tile of the Y region (= Kp / 256)
-    int tnb;             // B tiles of the Y region
+    int tiles_sym;       // number of 128 x 128 tiles covering the upper triangle of G (0 when G is not requested)
+    int tk;              // ceil(K / 128): row tiles
+    int tjx;             // ceil(K / 128): column tiles inside X
+    int tjy0;            // first column tile of the Y region (= Kp / 128)
+    int tnb;             // column tiles of the Y region
     int ntiles;
     int mtot;            // operand rows of one half (hi); the lo half starts at row mtot
 };
 
-// item -> (tile, split) -> (ti, tJ); the tiles of the upper triangle first (row ti: tJ = ti/2 .. tjx-1), then X'Y
+// tile index -> (ti, tj): the tiles of the upper triangle first (row ti: tj = ti .. tjx-1), then X'Y
+__host__ __device__ __forceinline__ void decode_tile(int l, int tiles_sym, int tjx, int tjy0, int tnb, int &ti, int &tj) {
+    if (l < tiles_sym) {
+        ti = 0;
+        while (l >= tjx - ti) { l -= tjx - ti; ++ti; }
+        tj = ti + l;
+    } else {
+        l -= tiles_sym;
+        ti = l / tnb;
+        tj = tjy0 + (l - ti * tnb);
+    }
+}
+
+// item -> (tile, split) -> (ti, tj)
 struct Item {
     int tile, split, ti, tj, nst;
     int64_t r_begin;
-    bool diag;  // the A rows are part of the B tile (ti / 2 == tJ inside X)
+    bool diag;  // ti == tj inside X: the A rows are the B rows
 };
-template <bool PAIR>
 __device__ __forceinline__ Item decode_item(const Tc2Params &P, int w) {
     Item it;
     it.split = w / P.ntiles;
     it.tile = w - it.split * P.ntiles;
-    int l = it.tile;
-    if (l < P.tiles_sym) {
-        int ti = 0;
-        if (PAIR) {  // 256 x 256 tiles: row ti holds tJ = ti .. tjx-1
-            while (l >= P.tjx - ti) { l -= P.tjx - ti; ++ti; }
-            it.tj = ti + l;
-        } else {     // 128 x 256 tiles: row ti holds tJ = ti/2 .. tjx-1
-            while (l >= P.tjx - (ti >> 1)) { l -= P.tjx - (ti >> 1); ++ti; }
-            it.tj = (ti >> 1) + l;
-        }
-        it.ti = ti;
-        it.diag = (l == 0);
-    } else {
-        l -= P.tiles_sym;
-        it.ti = l / P.tnb;
-        it.tj = P.tjy0 + (l - it.ti * P.tnb);
-        it.diag = false;
-    }
+    decode_tile(it.tile, P.tiles_sym, P.tjx, P.tjy0, P.tnb, it.ti, it.tj);
+    it.diag = it.tile < P.tiles_sym && it.ti == it.tj;
     it.r_begin = (int64_t)it.split * P.rows_per_split;
     int64_t r_end = it.r_begin + P.rows_per_split;
     if (r_end > P.Np) r_end = P.Np;
@@ -117,310 +89,41 @@ __device__ __forceinline__ Item decode_item(const Tc2Params &P, int w) {
 }
 
 // ------------------------------------------------------------------ the GEMM
+// Persistent grid (one CTA per SM), static round-robin over (output tile, row split) items; the TMA -> wgmma pipeline
+// of tc_common.cuh, one fp32 partial tile per item.
+// Bound: L2 -> SM operand traffic (64 KB per 3 x 128 x 128 x 64 products), then the tensor pipe.
 __global__ void __launch_bounds__(NTHREADS, 1)
-gram_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const Tc2Params P) {
+gram_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const Tc2Params P) {
     extern __shared__ unsigned char smem_dyn[];
     unsigned char *smem = (unsigned char *)(((uintptr_t)smem_dyn + 1023) & ~(uintptr_t)1023);
     const uint32_t sbase = smem_u32(smem);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int nitems = P.ntiles * P.nsplit;
-
-    auto bar = [&](int i) { return sbase + OFF_BAR + 8 * i; };
-    constexpr int FULL = 0, EMPTY = STAGES, ACC_FULL = 2 * STAGES, ACC_EMPTY = 2 * STAGES + 2;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(smem + OFF_TMEM);
-
-    if (threadIdx.x == T_TMA) {
-        for (int s = 0; s < STAGES; ++s) {
-            mbar_init(bar(FULL + s), 1);
-            mbar_init(bar(EMPTY + s), 1);
-        }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(bar(ACC_FULL + a), 1);
-            mbar_init(bar(ACC_EMPTY + a), NDRAIN_WARPS);
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == W_MMA) {  // all 512 TMEM columns: two fp32 accumulators of 256 columns
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
-
+    pipe_init(sbase);
+    uint32_t g = 0;
     if (warp == W_TMA) {
-        // ===================== TMA producer =====================
-        if (lane == 0) {
-            uint32_t g = 0;  // stages issued so far
+        if (lane == 0)
             for (int w = blockIdx.x; w < nitems; w += gridDim.x) {
-                const Item it = decode_item<false>(P, w);
-                const int rowA = it.ti * TM, rowB = it.tj * TN;
-                for (int st = 0; st < it.nst; ++st, ++g) {
-                    const int s = g % STAGES;
-                    const uint32_t ph = (g / STAGES) & 1;
-                    mbar_wait(bar(EMPTY + s), ph ^ 1);
-                    const uint32_t dst = sbase + s * STAGE_BYTES;
-                    const int r0 = (int)(it.r_begin + (int64_t)st * KS);
-                    mbar_arrive_expect_tx(bar(FULL + s), it.diag ? 2 * B_TILE : STAGE_BYTES);
-                    if (!it.diag) {
-                        tma_load_2d(dst, &mapA, bar(FULL + s), r0, rowA);
-                        tma_load_2d(dst + A_TILE, &mapA, bar(FULL + s), r0, P.mtot + rowA);
-                    }
-                    tma_load_2d(dst + 2 * A_TILE, &mapB, bar(FULL + s), r0, rowB);
-                    tma_load_2d(dst + 2 * A_TILE + B_TILE, &mapB, bar(FULL + s), r0, P.mtot + rowB);
-                }
+                const Item it = decode_item(P, w);
+                pipe_produce(sbase, g, &mapA, &mapA, it.ti * TILE, P.mtot, it.tj * TILE, P.mtot, it.r_begin, it.nst, it.diag);
             }
-        }
-    } else if (warp == W_MMA) {
-        // ===================== MMA issuer =====================
-        if (lane == 0) {
-            // instruction descriptor: D fp32 (1 << 4), A and B fp16 (format 0), both K-major, N >> 3 at 17, M >> 4 at 24
-            const uint32_t idesc = (1u << 4) | ((uint32_t)(TN >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
-            uint32_t g = 0, gc = 0;  // stages / accumulator runs so far
-            for (int w = blockIdx.x; w < nitems; w += gridDim.x) {
-                const Item it = decode_item<false>(P, w);
-                for (int st = 0; st < it.nst; ++st, ++g) {
-                    const int s = g % STAGES;
-                    const uint32_t ph = (g / STAGES) & 1;
-                    const int kk = st % SUB_STAGES;
-                    const uint32_t ab = gc & 1;
-                    if (kk == 0) mbar_wait(bar(ACC_EMPTY + ab), ((gc >> 1) & 1) ^ 1);  // accumulator drained
-                    mbar_wait(bar(FULL + s), ph);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const uint32_t stage = sbase + s * STAGE_BYTES;
-                    const uint32_t b_hi = stage + 2 * A_TILE, b_lo = b_hi + B_TILE;
-                    const uint32_t a_hi = it.diag ? b_hi + (uint32_t)(it.ti & 1) * A_TILE : stage;
-                    const uint32_t a_lo = it.diag ? b_lo + (uint32_t)(it.ti & 1) * A_TILE : stage + A_TILE;
-                    const uint32_t acc = tmem_base + ab * TN;
-#pragma unroll
-                    for (int ks = 0; ks < KS / 16; ++ks) {
-                        const uint32_t off = ks * 32;  // 16 fp16 = 32 bytes along K inside the 128-byte swizzled row
-                        const uint32_t first = (kk == 0 && ks == 0) ? 0u : 1u;
-                        umma_f16_ss(acc, umma_desc_k_sw128(a_hi + off), umma_desc_k_sw128(b_hi + off), idesc, first);
-                        umma_f16_ss(acc, umma_desc_k_sw128(a_hi + off), umma_desc_k_sw128(b_lo + off), idesc, 1u);
-                        umma_f16_ss(acc, umma_desc_k_sw128(a_lo + off), umma_desc_k_sw128(b_hi + off), idesc, 1u);
-                    }
-                    umma_commit(bar(EMPTY + s));  // stage free once these MMAs have read it
-                    if (kk == SUB_STAGES - 1 || st == it.nst - 1) {
-                        umma_commit(bar(ACC_FULL + ab));
-                        ++gc;
-                    }
-                }
-            }
-        }
-    } else {
-        // ===================== drain warps =====================
-        // thread -> accumulator row m (TMEM lane; a warp reaches the lanes of its quadrant, warp % 4) x 128 columns
-        const int quad = warp & 3, half = warp >> 2;
-        const int m = quad * 32 + lane;
-        const uint32_t lane_addr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(half * 128);
-        uint32_t gc = 0;
-        for (int w = blockIdx.x; w < nitems; w += gridDim.x) {
-            const Item it = decode_item<false>(P, w);
-            const int nsub = (it.nst + SUB_STAGES - 1) / SUB_STAGES;
-            float accv[128];
-#pragma unroll
-            for (int e = 0; e < 128; ++e) accv[e] = 0.f;
-            for (int c = 0; c < nsub; ++c, ++gc) {
-                const uint32_t ab = gc & 1;
-                mbar_wait(bar(ACC_FULL + ab), (gc >> 1) & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-                for (int gq = 0; gq < 2; ++gq) {
-                    uint32_t r0[32], r1[32];
-                    tmem_ld32(lane_addr + ab * TN + (uint32_t)(gq * 64), r0);
-                    tmem_ld32(lane_addr + ab * TN + (uint32_t)(gq * 64 + 32), r1);
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                    for (int e = 0; e < 32; ++e) {
-                        accv[gq * 64 + e] = __fadd_rn(accv[gq * 64 + e], __uint_as_float(r0[e]));
-                        accv[gq * 64 + 32 + e] = __fadd_rn(accv[gq * 64 + 32 + e], __uint_as_float(r1[e]));
-                    }
-                }
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                __syncwarp();
-                if (lane == 0) mbar_arrive(bar(ACC_EMPTY + ab));
-            }
-            float *dst = P.partial + ((size_t)it.split * P.ntiles + it.tile) * (size_t)(TM * TN) + (size_t)m * TN + half * 128;
-#pragma unroll
-            for (int e = 0; e < 128; e += 4)
-                *reinterpret_cast<float4 *>(dst + e) = make_float4(accv[e], accv[e + 1], accv[e + 2], accv[e + 3]);
-        }
+        return;
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == W_MMA) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512));
-    }
-}
-
-// ------------------------------------------------------------------ the GEMM, CTA-pair version (cta_group::2)
-// Two CTAs of a cluster (one TPC) compute one 256 x 256 tile: UMMA M = 256 (128 accumulator rows in the tensor memory
-// of each CTA), N = 256 with each CTA holding half of the B rows in ITS shared memory.  Per CTA and 64-row stage:
-// A hi/lo (own 128 rows) + B hi/lo (own 128 of the 256 B rows) = 64 KB for the same 1536 tensor-pipe cycles -- two
-// thirds of the operand traffic of the single-CTA tile -- which also makes room for a third stage.
-//   both CTAs   TMA producer (cp.async.bulk.tensor ... cta_group::2: complete_tx lands on the LEADER's full barrier),
-//               8 drain warps (own accumulator rows), arrive on the leader's accumulator-empty barrier
-//   leader      expect_tx for both CTAs' bytes, single-thread MMA issuer, commits multicast to both CTAs
-constexpr int PS_TILE = 128 * 128;                 // bytes of one 128-row operand tile (hi or lo)
-constexpr int PS_STAGE_BYTES = 4 * PS_TILE;        // A hi, A lo, B-half hi, B-half lo
-constexpr int PS_STAGES = 3;
-constexpr int PS_OFF_BAR = PS_STAGES * PS_STAGE_BYTES;
-constexpr int PS_NBAR = 2 * PS_STAGES + 4;
-constexpr int PS_OFF_TMEM = PS_OFF_BAR + PS_NBAR * 8;
-constexpr int PS_SMEM_BYTES = PS_OFF_TMEM + 16 + 1024;
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NTHREADS, 1)
-gram_tc2_pair_kernel(const __grid_constant__ CUtensorMap mapA, const Tc2Params P) {
-    extern __shared__ unsigned char smem_dyn[];
-    // both CTAs of the pair must use the same shared-memory offsets: the dynamic segment starts at the same offset in
-    // every CTA of a launch, so the aligned base is the same too
-    unsigned char *smem = (unsigned char *)(((uintptr_t)smem_dyn + 1023) & ~(uintptr_t)1023);
-    const uint32_t sbase = smem_u32(smem);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const bool leader = rank == 0;
-    const int ncl = gridDim.x >> 1, cid = blockIdx.x >> 1;
-    const int nitems = P.ntiles * P.nsplit;
-
-    auto bar = [&](int i) { return sbase + PS_OFF_BAR + 8 * i; };
-    constexpr int FULL = 0, EMPTY = PS_STAGES, ACC_FULL = 2 * PS_STAGES, ACC_EMPTY = 2 * PS_STAGES + 2;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(smem + PS_OFF_TMEM);
-
-    if (threadIdx.x == T_TMA) {
-        for (int s = 0; s < PS_STAGES; ++s) {
-            mbar_init(bar(FULL + s), 1);
-            mbar_init(bar(EMPTY + s), 1);
-        }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(bar(ACC_FULL + a), 1);
-            mbar_init(bar(ACC_EMPTY + a), 2 * NDRAIN_WARPS);  // the drain warps of both CTAs
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == W_MMA) {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    cluster_sync_all();  // barriers of both CTAs initialised before any remote arrive / multicast commit
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == W_TMA) {
-        // ===================== TMA producer (both CTAs) =====================
-        if (lane == 0) {
-            uint32_t g = 0;
-            for (int w = cid; w < nitems; w += ncl) {
-                const Item it = decode_item<true>(P, w);
-                const int rowA = it.ti * 256 + (int)rank * 128, rowB = it.tj * 256 + (int)rank * 128;
-                for (int st = 0; st < it.nst; ++st, ++g) {
-                    const int s = g % PS_STAGES;
-                    const uint32_t ph = (g / PS_STAGES) & 1;
-                    mbar_wait(bar(EMPTY + s), ph ^ 1);
-                    const uint32_t dst = sbase + s * PS_STAGE_BYTES;
-                    const uint32_t lbar = mapa_rank(bar(FULL + s), 0);
-                    const int r0 = (int)(it.r_begin + (int64_t)st * KS);
-                    if (leader) mbar_arrive_expect_tx(bar(FULL + s), 2 * (it.diag ? 2 * PS_TILE : PS_STAGE_BYTES));
-                    if (!it.diag) {
-                        tma_load_2d_pair(dst, &mapA, lbar, r0, rowA);
-                        tma_load_2d_pair(dst + PS_TILE, &mapA, lbar, r0, P.mtot + rowA);
-                    }
-                    tma_load_2d_pair(dst + 2 * PS_TILE, &mapA, lbar, r0, rowB);
-                    tma_load_2d_pair(dst + 3 * PS_TILE, &mapA, lbar, r0, P.mtot + rowB);
-                }
-            }
-        }
-    } else if (warp == W_MMA) {
-        // ===================== MMA issuer (leader CTA only) =====================
-        if (leader && lane == 0) {
-            const uint32_t idesc = (1u << 4) | ((uint32_t)(256 >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-            uint32_t g = 0, gc = 0;
-            for (int w = cid; w < nitems; w += ncl) {
-                const Item it = decode_item<true>(P, w);
-                for (int st = 0; st < it.nst; ++st, ++g) {
-                    const int s = g % PS_STAGES;
-                    const uint32_t ph = (g / PS_STAGES) & 1;
-                    const int kk = st % SUB_STAGES;
-                    const uint32_t ab = gc & 1;
-                    if (kk == 0) mbar_wait(bar(ACC_EMPTY + ab), ((gc >> 1) & 1) ^ 1);
-                    mbar_wait(bar(FULL + s), ph);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const uint32_t stage = sbase + s * PS_STAGE_BYTES;
-                    const uint32_t b_hi = stage + 2 * PS_TILE, b_lo = stage + 3 * PS_TILE;
-                    // diagonal tile: the A rows of each CTA are exactly its half of the B rows
-                    const uint32_t a_hi = it.diag ? b_hi : stage, a_lo = it.diag ? b_lo : stage + PS_TILE;
-                    const uint32_t acc = tmem_base + ab * 256;
+    const int wg = warp >> 2;
+    for (int w = blockIdx.x; w < nitems; w += gridDim.x) {
+        const Item it = decode_item(P, w);
+        float sum[FRAG];
+        pipe_consume(sbase, g, wg, it.nst, it.diag, sum);
+        float *dst = P.partial + ((size_t)it.split * P.ntiles + it.tile) * (size_t)(TILE * TN) + (size_t)(wg * 64) * TN;
 #pragma unroll
-                    for (int ks = 0; ks < KS / 16; ++ks) {
-                        const uint32_t off = ks * 32;
-                        const uint32_t first = (kk == 0 && ks == 0) ? 0u : 1u;
-                        umma_f16_ss_pair(acc, umma_desc_k_sw128(a_hi + off), umma_desc_k_sw128(b_hi + off), idesc, first);
-                        umma_f16_ss_pair(acc, umma_desc_k_sw128(a_hi + off), umma_desc_k_sw128(b_lo + off), idesc, 1u);
-                        umma_f16_ss_pair(acc, umma_desc_k_sw128(a_lo + off), umma_desc_k_sw128(b_hi + off), idesc, 1u);
-                    }
-                    umma_commit_pair(bar(EMPTY + s));
-                    if (kk == SUB_STAGES - 1 || st == it.nst - 1) {
-                        umma_commit_pair(bar(ACC_FULL + ab));
-                        ++gc;
-                    }
-                }
-            }
-        }
-    } else {
-        // ===================== drain warps (both CTAs, own 128 accumulator rows) =====================
-        const int quad = warp & 3, half = warp >> 2;
-        const int m = quad * 32 + lane;
-        const uint32_t lane_addr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(half * 128);
-        uint32_t gc = 0;
-        for (int w = cid; w < nitems; w += ncl) {
-            const Item it = decode_item<true>(P, w);
-            const int nsub = (it.nst + SUB_STAGES - 1) / SUB_STAGES;
-            float accv[128];
-#pragma unroll
-            for (int e = 0; e < 128; ++e) accv[e] = 0.f;
-            for (int c = 0; c < nsub; ++c, ++gc) {
-                const uint32_t ab = gc & 1;
-                mbar_wait(bar(ACC_FULL + ab), (gc >> 1) & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-                for (int gq = 0; gq < 2; ++gq) {
-                    uint32_t r0[32], r1[32];
-                    tmem_ld32(lane_addr + ab * 256 + (uint32_t)(gq * 64), r0);
-                    tmem_ld32(lane_addr + ab * 256 + (uint32_t)(gq * 64 + 32), r1);
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                    for (int e = 0; e < 32; ++e) {
-                        accv[gq * 64 + e] = __fadd_rn(accv[gq * 64 + e], __uint_as_float(r0[e]));
-                        accv[gq * 64 + 32 + e] = __fadd_rn(accv[gq * 64 + 32 + e], __uint_as_float(r1[e]));
-                    }
-                }
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                __syncwarp();
-                if (lane == 0) mbar_arrive_cluster(mapa_rank(bar(ACC_EMPTY + ab), 0));
-            }
-            float *dst = P.partial + ((size_t)it.split * P.ntiles + it.tile) * (size_t)(256 * 256) +
-                         (size_t)(rank * 128 + m) * 256 + half * 128;
-#pragma unroll
-            for (int e = 0; e < 128; e += 4)
-                *reinterpret_cast<float4 *>(dst + e) = make_float4(accv[e], accv[e + 1], accv[e + 2], accv[e + 3]);
-        }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    cluster_sync_all();  // neither CTA leaves (or frees tensor memory) while the other may still touch it
-    if (warp == W_MMA) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512));
+        for (int e = 0; e < FRAG; e += 2)
+            *reinterpret_cast<float2 *>(dst + (size_t)frag_row(e) * TN + frag_col(e)) = make_float2(sum[e], sum[e + 1]);
     }
 }
 
 // ------------------------------------------------------------------ operand space
 // Operand row o of the GEMM: o < Kp -> column o of X (zero row when o >= K); o >= Kp -> column o - Kp of Y.
-// Kp and the Y extent are multiples of 256, so no strip of the kernels below straddles the two matrices.
+// Kp and the Y extent are multiples of 128, so no strip of the kernels below straddles the two matrices.
 struct Cols {
     const float *X, *Y;
     int64_t ldx, ldy;
@@ -647,36 +350,22 @@ tc2_stat_finish(const double *__restrict__ part, const double *__restrict__ part
 }
 
 // ------------------------------------------------------------------ reduction of the row splits
-// CTA = 32 rows x 128 columns (one 128-column block) of a tile; thread = 4 consecutive columns x 4 rows (float4 loads of
-// every split's partial, all issued before the first use).
+// CTA = 32 rows x 128 columns of a tile; thread = 4 consecutive columns x 4 rows (float4 loads of every split's partial,
+// all issued before the first use).
 //   C[i,j] = inv_i inv_j sum_s P_s[i,j] + uA_i TB_j + TA_i uB_j + N uA_i uB_j,   u = (double)shift32 - bias.
-// G tiles: 128-blocks below the diagonal block are skipped, the diagonal 128-block reads the upper element for both
-// (i,j) and (j,i) (the tensor core produced them with different rounding; G must be bitwise symmetric), blocks above
-// it are also written transposed (the lower triangle of G) through shared memory.  TR = rows of a tile (128, or 256
-// for the pair kernel).
-template <int TR>
+// G tiles: the diagonal tile reads the upper element for both (i,j) and (j,i) (the tensor core produced them with
+// different rounding; G must be bitwise symmetric), tiles above it are also written transposed (the lower triangle of G)
+// through shared memory.
 __global__ void __launch_bounds__(256)
 reduce_tc2(const float *__restrict__ partial, int nsplit, int ntiles, int tiles_sym, int tjx, int tjy0, int tnb, int Kp,
            const float *__restrict__ shift, const double *__restrict__ inv, const double *__restrict__ T,
            const double *__restrict__ SQ, const float *__restrict__ y_bias, double Nd, int K, int n,
            double *__restrict__ G, double *__restrict__ Bxy) {
+    constexpr int TR = TILE;
     __shared__ double tr[32][129];
-    int l = blockIdx.x, ti, tj;
-    const bool sym = l < tiles_sym;
-    if (sym) {
-        ti = 0;
-        if (TR == 128) {
-            while (l >= tjx - (ti >> 1)) { l -= tjx - (ti >> 1); ++ti; }
-            tj = (ti >> 1) + l;
-        } else {
-            while (l >= tjx - ti) { l -= tjx - ti; ++ti; }
-            tj = ti + l;
-        }
-    } else {
-        l -= tiles_sym;
-        ti = l / tnb;
-        tj = tjy0 + (l - ti * tnb);
-    }
+    int ti, tj;
+    const bool sym = (int)blockIdx.x < tiles_sym;
+    decode_tile(blockIdx.x, tiles_sym, tjx, tjy0, tnb, ti, tj);
     const int rowbase = ti * TR, colbase = tj * TN;  // colbase in operand space
     const int sr = blockIdx.y, i0 = rowbase + sr * 32;
     if (i0 >= K) return;
@@ -789,10 +478,12 @@ reduce_tc2(const float *__restrict__ partial, int nsplit, int ntiles, int tiles_
 
 }  // namespace
 
-// CPB200_GRAM_PAIR=0 selects the single-CTA 128 x 256 tiles (A/B measurements); default: CTA pairs, 256 x 256 tiles
-static bool tc2_use_pair() {
-    static const bool pair = [] { const char *e = getenv("CPB200_GRAM_PAIR"); return !(e && e[0] == '0'); }();
-    return pair;
+bool cp_gram_tc_eligible(const float *X, int64_t N, int K, int64_t ldx, const void *Yraw, int y_dtype, int n, int64_t ldy,
+                         const int32_t *rows, bool wantB) {
+    if (rows != nullptr || N < 64 || K < 64) return false;
+    if ((((uintptr_t)X) & 15) || (ldx % 4)) return false;  // 16-byte vector loads of the statistics / preparation passes
+    if (wantB && (y_dtype != CP_F32 || (((uintptr_t)Yraw) & 15) || (ldy % 4) || n < 1)) return false;
+    return true;
 }
 
 int cp_gram_tc2(cp_handle_t h, const float *X, int64_t N, int K, int64_t ldx, const void *Yraw, int y_dtype, int n,
@@ -803,25 +494,23 @@ int cp_gram_tc2(cp_handle_t h, const float *X, int64_t N, int K, int64_t ldx, co
         return cp_gram_fp64_products(h, X, N, K, ldx, Yraw, y_dtype, n, ldy, y_bias, rows, nrows, G, Bxy, sx, sy, yy, stream);
     if (sy != nullptr && !wantB)  // column sums of Y alone: nothing for the tensor cores to do
         return cp_gram_fp64_products(h, X, N, K, ldx, Yraw, y_dtype, n, ldy, y_bias, rows, nrows, G, Bxy, sx, sy, yy, stream);
-    const bool pair = tc2_use_pair();
-    const int TR = pair ? 256 : TM;
-    const int tjx = cp_cdiv(K, TN), tk = cp_cdiv(K, TR);
+    const int tjx = cp_cdiv(K, TN), tk = tjx;
     const int Kp = tjx * TN;
     const int tnb = wantB ? cp_cdiv(n, TN) : 0;
     const int np_ = tnb * TN;
     const int mtot = Kp + np_;
     int tiles_sym = 0;
     if (G)
-        for (int ti = 0; ti < tk; ++ti) tiles_sym += pair ? tjx - ti : tjx - (ti >> 1);
+        tiles_sym = tk * (tk + 1) / 2;
     const int ntiles = tiles_sym + tk * tnb;
     const int64_t Np = cp_cdiv(N, KS) * (int64_t)KS;
-    const int units = pair ? h->num_sms / 2 : h->num_sms;  // CTAs or CTA pairs working concurrently
+    const int units = h->num_sms;  // CTAs working concurrently
 
     // Row splits.  An item (tile x split) costs its stages (~1.2 us each) plus a small hand-over; items run
     // round-robin on the persistent grid; every split adds one fp32 partial per tile (written, then read by the
-    // reduction).  A split is a multiple of the 128-row accumulator run and at most 32 runs (the fp32 register
-    // sums stay below 4e-7 of the partial sum whatever N is).
-    constexpr int64_t SUB = SUB_STAGES * KS, MAX_SPLIT_ROWS = 32 * SUB;
+    // reduction).  A split is a multiple of the accumulator run and at most 4096 rows (the fp32 register sums
+    // stay below 4e-7 of the partial sum whatever N is).
+    constexpr int64_t SUB = SUB_STAGES * KS, MAX_SPLIT_ROWS = 4096;
     const int ns_min = (int)cp_cdiv(N, MAX_SPLIT_ROWS);
     int nsplit = ns_min, rps = (int)(cp_cdiv(cp_cdiv(N, ns_min), SUB) * SUB);
     if (ntiles > 0) {
@@ -832,7 +521,7 @@ int cp_gram_tc2(cp_handle_t h, const float *X, int64_t N, int K, int64_t ldx, co
             const int ns_eff = (int)cp_cdiv(N, r);
             const double rounds = (double)cp_cdiv((int64_t)ntiles * ns_eff, units);
             const double cost = rounds * (1.2 * (double)(r / KS) + 1.0) +
-                                (double)ns_eff * (2.0 * ntiles * TR * TN * 4.0 / 5.0e6);
+                                (double)ns_eff * (2.0 * ntiles * TILE * TN * 4.0 / 3.0e6);  // HBM bytes per us
             if (cost < best * 0.98) {
                 best = cost;
                 nsplit = ns_eff;
@@ -841,7 +530,7 @@ int cp_gram_tc2(cp_handle_t h, const float *X, int64_t N, int K, int64_t ldx, co
         }
     }
 
-    const size_t part_elems = (size_t)nsplit * ntiles * TR * TN;
+    const size_t part_elems = (size_t)nsplit * ntiles * TILE * TN;
     const size_t op_elems = 2 * (size_t)mtot * (size_t)Np;  // hi rows, then lo rows
     const size_t need = cp_carver::need(part_elems, 4) + cp_carver::need(op_elems, 2) + 3 * cp_carver::need(mtot, 8) +
                         2 * cp_carver::need((size_t)RS * mtot, 8) + cp_carver::need((size_t)RS * mtot, 4) +
@@ -874,8 +563,8 @@ int cp_gram_tc2(cp_handle_t h, const float *X, int64_t N, int K, int64_t ldx, co
                                                             wantB ? sy : nullptr);
     CP_CHECK_LAUNCH();
     if (ntiles > 0) {
-        CUtensorMap mapA, mapB;
-        rc = make_map16(h, &mapA, ops, Np, 2 * (int64_t)mtot, TM);
+        CUtensorMap mapA;
+        rc = make_map16(h, &mapA, ops, Np, 2 * (int64_t)mtot, TILE);
         if (rc) return rc;
         Tc2Params P{};
         P.partial = partial; P.Np = Np; P.rows_per_split = rps; P.nsplit = nsplit; P.tiles_sym = tiles_sym; P.tk = tk;
@@ -883,33 +572,17 @@ int cp_gram_tc2(cp_handle_t h, const float *X, int64_t N, int K, int64_t ldx, co
         const int nitems = ntiles * nsplit;
         const bool prof = h->gram_profile;
         if (prof) CP_CUDA(cudaEventRecord(h->ev_gram0, stream));
-        if (pair) {
-            static cp_per_device_flag configured;
-            if (bool *done = configured.slot(); !*done) {
-                CP_CUDA(cudaFuncSetAttribute(gram_tc2_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PS_SMEM_BYTES));
-                *done = true;
-            }
-            const int ncl = nitems < units ? nitems : units;
-            gram_tc2_pair_kernel<<<2 * ncl, NTHREADS, PS_SMEM_BYTES, stream>>>(mapA, P);
-        } else {
-            rc = make_map16(h, &mapB, ops, Np, 2 * (int64_t)mtot, TN);
-            if (rc) return rc;
-            static cp_per_device_flag configured;
-            if (bool *done = configured.slot(); !*done) {
-                CP_CUDA(cudaFuncSetAttribute(gram_tc2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-                *done = true;
-            }
-            const int grid = nitems < units ? nitems : units;
-            gram_tc2_kernel<<<grid, NTHREADS, SMEM_BYTES, stream>>>(mapA, mapB, P);
+        static cp_per_device_flag configured;
+        if (bool *done = configured.slot(); !*done) {
+            CP_CUDA(cudaFuncSetAttribute(gram_tc2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+            *done = true;
         }
+        const int grid = nitems < units ? nitems : units;
+        gram_tc2_kernel<<<grid, NTHREADS, SMEM_BYTES, stream>>>(mapA, P);
         CP_CHECK_LAUNCH();
         if (prof) CP_CUDA(cudaEventRecord(h->ev_gram1, stream));
-        if (pair)
-            reduce_tc2<256><<<dim3(ntiles, 8, 2), 256, 0, stream>>>(partial, nsplit, ntiles, tiles_sym, tjx, P.tjy0, tnb, Kp, shift,
-                                                                   inv, T, SQ, y_bias, Nd, K, n, G, Bxy);
-        else
-            reduce_tc2<128><<<dim3(ntiles, 4, 2), 256, 0, stream>>>(partial, nsplit, ntiles, tiles_sym, tjx, P.tjy0, tnb, Kp, shift,
-                                                                   inv, T, SQ, y_bias, Nd, K, n, G, Bxy);
+        reduce_tc2<<<dim3(ntiles, TILE / 32, TN / 128), 256, 0, stream>>>(partial, nsplit, ntiles, tiles_sym, tjx, P.tjy0, tnb, Kp,
+                                                                         shift, inv, T, SQ, y_bias, Nd, K, n, G, Bxy);
         CP_CHECK_LAUNCH();
     }
     return CP_OK;

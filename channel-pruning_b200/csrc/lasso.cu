@@ -160,25 +160,33 @@ __device__ __forceinline__ void wait_ge(const int *p, int target) {
     for (uint32_t spin = 0; ld_acquire(p) < target; ++spin)
         if (spin > (1u << 26)) __trap();
 }
-// progress hints (ring-reuse slack only; a stale value merely delays the waiter)
-__device__ __forceinline__ void wait_ge_relaxed(const int *p, int target) {
-    for (uint32_t spin = 0; *reinterpret_cast<const volatile int *>(p) < target; ++spin) {
+// ring-reuse positions: published with st_release after a __syncwarp, so that the reads of the slots they free are
+// ordered before the waiter's overwrite
+__device__ __forceinline__ void wait_ge_backoff(const int *p, int target) {
+    for (uint32_t spin = 0; ld_acquire(p) < target; ++spin) {
         if (spin > (1u << 26)) __trap();
         poll_backoff();
     }
 }
-// Tagged 16-byte records {value, tag}: written with ONE st.shared.v2.f64 and read with ONE ld.shared.v2.f64, so
-// value and tag always travel together -- no separate flag, no fence on the serial chain.
+// Tagged 16-byte records {value, check}: ONE st.shared.v2.f64 / ld.shared.v2.f64 each, no fence on the serial chain.
+// A vector access is not single-copy atomic, so check = value bits XOR a mix of the tag: a read that combines halves of
+// two records fails the check (unless both held the same value) and is repeated.
+__device__ __forceinline__ long long tag_mix(uint32_t tag) {
+    return (long long)(((uint64_t)tag * 0x9E3779B97F4A7C15ull) | 1ull);
+}
+__device__ __forceinline__ bool tag_ok(double v, double t, uint32_t tag) {
+    return (__double_as_longlong(v) ^ __double_as_longlong(t)) == tag_mix(tag);
+}
 __device__ __forceinline__ void put_tagged(uint32_t slot_saddr, double v, uint32_t tag) {
     asm volatile("st.volatile.shared.v2.f64 [%0], {%1, %2};" ::"r"(slot_saddr), "d"(v),
-                 "d"(__hiloint2double(0, (int)tag))
+                 "d"(__longlong_as_double(__double_as_longlong(v) ^ tag_mix(tag)))
                  : "memory");
 }
 __device__ __forceinline__ double get_tagged(uint32_t slot_saddr, uint32_t tag) {
     double v, t;
     for (uint32_t spin = 0;; ++spin) {
         asm volatile("ld.volatile.shared.v2.f64 {%0, %1}, [%2];" : "=d"(v), "=d"(t) : "r"(slot_saddr) : "memory");
-        if ((uint32_t)__double2loint(t) == tag) break;
+        if (tag_ok(v, t, tag)) break;
         if (spin > (1u << 26)) __trap();
     }
     return v;
@@ -189,7 +197,7 @@ __device__ __forceinline__ double wait_tagged(uint32_t slot_saddr, uint32_t tag)
     double v, t;
     for (uint32_t spin = 0;; ++spin) {
         asm volatile("ld.volatile.shared.v2.f64 {%0, %1}, [%2];" : "=d"(v), "=d"(t) : "r"(slot_saddr) : "memory");
-        if ((uint32_t)__double2loint(t) == tag) break;
+        if (tag_ok(v, t, tag)) break;
         if (spin > (1u << 24)) __trap();
         poll_backoff();
     }
@@ -269,7 +277,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) lasso_select_kernel(const Selec
         excluded[e] = 0;
     }
     for (int e = tid; e < RING * CP; e += WS_THREADS) ring[e] = 0.0;  // padding pairs stay zero
-    for (int e = tid; e < QR * 4; e += WS_THREADS) dq[e] = 0.0;        // dq and xq: tag 0 never matches
+    for (int e = tid; e < QR * 4; e += WS_THREADS) dq[e] = 0.0;        // dq and xq: no tag matches {0, 0}
     __syncthreads();
     uint32_t sweep_no = 1;  // tags are (sweep_no << 12) | (step + 1): unique over the whole launch (< 2^20 sweeps)
 
@@ -433,10 +441,11 @@ __global__ void __launch_bounds__(WS_THREADS, 1) lasso_select_kernel(const Selec
             auto block_sync = [&](int s0) {  // before any step of s0 .. s0+15 or the fetch of s0+16
                 wait_ge(&ctl.pk_pos, s0 + 17 < n_active ? s0 + 17 : n_active);
                 // operands of steps <= s0 are in registers: their slots may be reused
-                if (lane == 0) *reinterpret_cast<volatile int *>(&ctl.chain_pos) = s0;
+                __syncwarp();
+                if (lane == 0) st_release(&ctl.chain_pos, s0);
                 if (s0 >= 32) {  // nobody may fall more than ~32 steps behind (ring reuse)
 #pragma unroll
-                    for (int b = 0; b < NBULK; ++b) wait_ge_relaxed(&ctl.bulk_pos[b], s0 - 24);
+                    for (int b = 0; b < NBULK; ++b) wait_ge_backoff(&ctl.bulk_pos[b], s0 - 24);
                 }
             };
             auto run_block = [&](auto guarded, int s0) {
@@ -455,7 +464,10 @@ __global__ void __launch_bounds__(WS_THREADS, 1) lasso_select_kernel(const Selec
                     const uint32_t tag = tag0 + (uint32_t)(s + 1);
                     const uint32_t j = J[cur];
                     double xv = XV[cur];
-                    if ((uint32_t)__double2loint(XT[cur]) != tag) xv = get_tagged(xq_s + (uint32_t)(sb + i) * 16u, tag);
+                    if (!tag_ok(XV[cur], XT[cur], tag)) xv = get_tagged(xq_s + (uint32_t)(sb + i) * 16u, tag);
+                    // the lanes leave the spin above independently; w[] below is written by every lane and read back
+                    // by every lane one step later, so a lane must not run ahead of one still storing an older w[j]
+                    __syncwarp();
                     CH_STAMP(s, 2);
                     double x = xv;
 #pragma unroll
@@ -568,7 +580,10 @@ __global__ void __launch_bounds__(WS_THREADS, 1) lasso_select_kernel(const Selec
                     if (rec && b == 0 && lane == 0 && t < TSTEPS) cp_lasso_times[t * 8 + 7] = clock64();
 #endif
                 }
-                if ((DEPTH == 8 || (t0 & 4)) && lane == 0) *reinterpret_cast<volatile int *>(&ctl.bulk_pos[b]) = t0 + DEPTH;
+                if (DEPTH == 8 || (t0 & 4)) {
+                    __syncwarp();
+                    if (lane == 0) st_release(&ctl.bulk_pos[b], t0 + DEPTH);
+                }
             };
             for (int t0 = 0; t0 < n_active; t0 += DEPTH) {
                 if (t0 + DEPTH <= n_active) run_block(std::false_type{}, t0);
@@ -579,7 +594,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) lasso_select_kernel(const Selec
         } else if (role == NBULK) {
             // -------- packager: operands of 32 chain steps at a time
             for (int base = 0; base < n_active; base += 32) {
-                if (base >= QR) wait_ge_relaxed(&ctl.chain_pos, base - 32);  // slots of batch base-64 are free
+                if (base >= QR) wait_ge_backoff(&ctl.chain_pos, base - 32);  // slots of batch base-64 are free
                 const int s = base + lane;
                 if (s < n_active) {
                     const uint32_t j = jz[s];

@@ -33,7 +33,7 @@
 bool cp_gemm_tc_enabled();
 int cp_gemm_tc_f64(cp_handle_t h, int slot, const double *A, int64_t lda, const double *B, int64_t ldb, double *C,
                    int64_t ldc, int M, int Nn, int R, double alpha, double beta, int lower, cudaStream_t stream,
-                   int max_clusters, int b_nc);
+                   int max_ctas, int b_nc);
 
 namespace {
 
@@ -156,8 +156,8 @@ struct MmTask {
     MmTerm t[3];
 };
 // Block products on the FP64 tensor path: four warps per task, one 16 x 16 quadrant each (2 x 2 m8n8k4 tiles), so the
-// twelve warps of a three-task phase sit on all four schedulers (a 2 x 4 register micro-tile per thread on 128
-// threads per task took 40k cycles for the block inversion of a panel; profiles/r2_summary.md has the new figure).
+// twelve warps of a three-task phase sit on all four schedulers (rather than a 2 x 4 register micro-tile per thread on
+// 128 threads per task).
 // Fragment loads: A[r][q], B[c][q] with q contiguous (the MmTerm convention).
 __device__ __forceinline__ void run_tasks_mma(const MmTask *tasks, int ntask) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -474,13 +474,13 @@ int dgemm_big(const double *A, int64_t lda, const double *B, int64_t ldb, double
               cp_handle_t tc = nullptr) {
     using namespace cpgemm;
     // tensor-core handle given and enabled: split-precision product (gemm_tc.cu) for everything wide enough to fill
-    // 256 x 256 tiles; one operand buffer per stream of the solver
+    // its 128 x 128 tiles; one operand buffer per stream of the solver
     static const int tc_min_nn = [] { const char *e = getenv("CPB200_LS_TC_MIN_NN"); return e ? atoi(e) : 192; }();
     if (tc && tc->ls_tc && cp_gemm_tc_enabled() && R >= 128 && R <= 1024 && Nn >= tc_min_nn && M >= 256 &&
         (tile_mode == TILES_ALL || tile_mode == TILES_LOWER)) {
         const int slot = stream == tc->side ? 1 : (stream == tc->bulk ? 2 : 0);
         return cp_gemm_tc_f64(tc, slot, A, lda, B, ldb, C, ldc, M, Nn, (int)R, alpha, beta, tile_mode == TILES_LOWER, stream,
-                              max_ctas > 0 ? max_ctas / 2 : 0, 0);
+                              max_ctas, 0);
     }
     bool done = false;
     int rca = dgemm_async<128, false>(A, lda, B, ldb, C, ldc, M, Nn, R, alpha, beta, tile_mode, stream, max_ctas, &done);
@@ -519,6 +519,13 @@ int dgemm_small(const double *A, int64_t lda, const double *B, int64_t ldb, doub
 // The look-ahead stream runs one priority level below the stream of the first solve on this handle (a handle serves one
 // stream in the layer pipeline): behind its own chain, ahead of cheaper problems' work.
 // grid cap of the bulk trailing updates: two thirds of the SMs (CPB200_LS_REST_CTAS overrides; 0 = uncapped)
+int device_sms() {  // SMs of the current device
+    int d = 0, n = 0;
+    cudaGetDevice(&d);
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, d);
+    return n;
+}
+
 int rest_ctas(cp_handle_t h) {
     static const int env = [] { const char *e = getenv("CPB200_LS_REST_CTAS"); return e ? atoi(e) : -1; }();
     return env >= 0 ? env : h->num_sms * 2 / 3;
@@ -733,9 +740,9 @@ static int chol_forward(const double *L, int64_t ld, int Kd, const double *Xinv,
         if (rc) return rc;
         if (Kd - g1 > 0) {  // Zt[:, g1:] -= F_g * L[g1:, g0:g1]'
             // few right-hand sides: 128 x 128 tiles would leave most SMs idle on a 512-deep product, 64 x 64 tiles fill them
-            // tensor-core mode: 256 x 256 pair tiles (n >= 256 right-hand sides, a few column tiles) beat the fp64 pipe
+            // tensor-core mode: split-precision tiles (n >= 256 right-hand sides, a few column tiles) beat the fp64 pipe
             const bool use_tc = tc && tc->ls_tc && cp_gemm_tc_enabled() && n >= 256 && Kd - g1 >= 512;
-            if (use_tc || cpgemm::num_tiles(n, Kd - g1, cpgemm::TILES_ALL) >= 2 * 148)
+            if (use_tc || cpgemm::num_tiles(n, Kd - g1, cpgemm::TILES_ALL) >= 2 * device_sms())
                 rc = dgemm_big(F + g0, ldz, L + (int64_t)g1 * ld + g0, ld, Zt + g1, ldz, n, Kd - g1, gs, -1.0, 1.0,
                                cpgemm::TILES_ALL, stream, 0, use_tc ? tc : nullptr);
             else
@@ -759,7 +766,7 @@ static int chol_backward(const double *L, int64_t ld, int Kd, const double *Xinv
         if (rc) return rc;
         if (g0 > 0) {  // F[:, 0:g0] -= Wt_g * L[g0:g0+gs, 0:g0]
             const bool use_tc = tc && tc->ls_tc && cp_gemm_tc_enabled() && n >= 256 && g0 >= 512;
-            if (use_tc || cpgemm::num_tiles(n, g0, cpgemm::TILES_ALL) >= 2 * 148)
+            if (use_tc || cpgemm::num_tiles(n, g0, cpgemm::TILES_ALL) >= 2 * device_sms())
                 rc = dgemm_big_nc(Wt + g0, ldw, L + (int64_t)g0 * ld, ld, F, ldf, n, g0, gs, -1.0, 1.0, stream,
                                   use_tc ? tc : nullptr);
             else
@@ -985,7 +992,7 @@ extern "C" int cp_ls_residual(cp_handle_t h, const float *X, int64_t N, int K, i
     cudaStream_t stream = (cudaStream_t)stream_;
     if (mode == CP_GRAM_3XTF32 && N % 4 == 0 && N >= 128 && K >= 64 && n % 4 == 0) {
         // Tensor-core variant: X Wf' = (X')'(Wf') is a product of the cp_gram shape (reduction over the ROWS of both
-        // operands) once X is transposed: 3xTF32 on the tcgen05 pipe instead of 2 N K n flops on the FP64 pipe.  Its
+        // operands) once X is transposed: split precision on the tensor cores instead of 2 N K n flops on the FP64 pipe.  Its
         // ~4e-7 relative error in the prediction perturbs the correction ~sqrt(N) times less than the same relative
         // error in the Gram matrix did (the residual error is uncorrelated noise, not a structured change of G).
         const int64_t ldt = N;
@@ -1016,7 +1023,7 @@ extern "C" int cp_ls_residual(cp_handle_t h, const float *X, int64_t N, int K, i
     }
     const int64_t ldw = ld_for(K);
     // X Wf' in fp64 (exact products of fp32 data with the fp64 weights): 128 x 128 tiles, reduction split so that the
-    // tile count fills whole waves of the SMs (5000 x 512 is 160 tiles on 148 SMs: two waves for 1.08 waves of work)
+    // tile count fills whole waves of the SMs (5000 x 512 is 160 tiles on 132 SMs: two waves for 1.2 waves of work)
     const int tiles = num_tiles((int)N, n, TILES_ALL);
     int nsplit = 1;
     double best = 1e30;

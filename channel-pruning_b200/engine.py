@@ -23,19 +23,16 @@ from . import _cabi
 RAND_R_MAX = 2147483647
 MAX_PROBES = 64
 # Least squares from tensor-core (3xTF32) statistics: the ~4e-7 relative error of that Gram is amplified by the
-# conditioning of the system (profiles/r2_conditioning.md maps it: 5e-6 of relative weight error at a pivot ratio of
-# 0.2, 2e-4 at 0.01, 5e-3 at 1e-4), so every such solve is followed by ONE step of iterative refinement against the
+# conditioning of the system (profiles/conditioning_map.py maps the weight error against the pivot ratio), so every such solve is followed by ONE step of iterative refinement against the
 # same factor with the residual taken from the data (engine.ls_refine) -- which squares the error -- and is accepted
 # only while the smallest Cholesky pivot keeps at least LS_RATIO_MIN of its original diagonal entry (1 - R^2 of the
 # most collinear column); below that the layer is re-solved from exact-product fp64 statistics.
 LS_RATIO_MIN = float(os.environ.get("CPB200_LS_RATIO_MIN", "0.005"))
 LS_REFINE = os.environ.get("CPB200_LS_REFINE", "1") == "1"
 # Prediction X W' of the refinement residual: "fp64" (SIMT fp64 GEMM), "tc" (tensor cores, through cp_gram on the
-# transposed patches) or "auto" (tensor cores for N >= 20000 only).  With the first-generation 3xTF32 kernel "tc" was
-# a loss inside the 13-layer pipeline (59.6 vs 48.5 ms per step, profiles/r2_summary.md: one CTA per tile held a whole
-# SM's shared memory for ~70 us and the latency-bound chains of the other layers queued behind them).  The second-
-# generation kernel (gram_tc2.cu) is a ~100 us persistent launch: 32.1 vs 36.1 ms per step (call 19) -- the FP64 pipe
-# is the step's scarce resource and this takes 2NK'n flop per layer off it.  Default "tc" (in the tensor-core mode).
+# transposed patches) or "auto" (tensor cores for N >= 20000 only).  The tensor-core Gram (gram_tc2.cu) is one short
+# persistent launch, and the FP64 pipe is the step's scarce resource: "tc" takes 2NK'n flop per layer off it.
+# Default "tc" (in the tensor-core mode).
 LS_RESID = os.environ.get("CPB200_LS_RESID", "tc")
 LS_RESID_TC_MIN_N = 20000
 # Bulk products of the Cholesky solve on the tensor cores when the statistics came from there (cp_ls_tensor_cores)
@@ -43,7 +40,7 @@ LS_TC = os.environ.get("CPB200_LS_TC", "1") == "1"
 # Full Gram of a layer enqueued after its channel search, on a lowest-priority stream (select_channels_async)
 DEFER_FULL_GRAM = os.environ.get("CPB200_DEFER_GRAM", "1") == "1"
 
-_PRIO_HIGHEST = -5  # cudaDeviceGetStreamPriorityRange on B200: [0, -5]; out-of-range values are clamped by the runtime
+_PRIO_HIGHEST = -5  # cudaDeviceGetStreamPriorityRange on H100: [0, -5]; out-of-range values are clamped by the runtime
 _LAYOUTS = {"nchw": 0, "nhwc": 1}
 GRAM_FP64, GRAM_3XTF32 = 0, 1
 
@@ -125,9 +122,9 @@ class Engine:
                 self._handles.append(hp[0])
                 # The pipeline hands its most expensive problems to the first slots.  CPB200_STREAM_PRIORITY:
                 #   "1"      (default) two levels: the first half of the slots high
-                #   "graded" one level per slot from the highest down (B200: -5 .. 0)        "0"  none
-                # measured on the 13-layer step (profiles/r2_summary.md): 48.3 / 48.9 / 49.0 ms -- priorities only order
-                # CTAs that are not yet resident, and the step is bound by FP64 throughput, not by the order
+                #   "graded" one level per slot from the highest down (H100: -5 .. 0)        "0"  none
+                # priorities only order CTAs that are not yet resident, so they matter little when the step is bound
+                # by FP64 throughput
                 pol = os.environ.get("CPB200_STREAM_PRIORITY", "1")
                 if pol == "graded":
                     prio = min(0, _PRIO_HIGHEST + i)
@@ -598,8 +595,8 @@ class Engine:
         S = samples.numel()
         # The search needs only the channel-space statistics (Q from the sampled rows and W2); the full Gram feeds the
         # reconstruction.  In the pipeline (one stream per layer) it is therefore enqueued AFTER the search, on a
-        # lowest-priority stream with its own handle: the ~0.5 ms full-GPU launch no longer delays the start of this
-        # and of every later layer's 8 ms single-SM search, it runs in their shadow.
+        # lowest-priority stream with its own handle: the full-GPU launch no longer delays the start of this and of
+        # every later layer's single-SM search, it runs in their shadow.
         defer = DEFER_FULL_GRAM and self.streams[0] is not None
         if defer:
             cur = torch.cuda.current_stream(self.device)
@@ -647,7 +644,7 @@ class Engine:
             W, b, info, stat = self.ls_solve(g_full, cols_d)
             if g_full["mode"] != GRAM_FP64 and LS_REFINE:
                 # statistics from the 3xTF32 Gram carry ~4e-7 relative error, which the conditioning of a wide layer
-                # amplifies to ~4e-5 in W and more in b (measured at conv4_x, N=5000): one refinement step against
+                # amplifies by orders of magnitude in W and more in b: one refinement step against
                 # the same factor, with the residual taken from the data, restores fp64-level accuracy
                 self.ls_refine(g_full, X, Y, y_bias, cols_d, W, b)
             return W, b, info, stat

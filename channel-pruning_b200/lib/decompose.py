@@ -1,7 +1,7 @@
 """Drop-in for the channel-pruning part of the reference's ``lib/decompose.py``.
 
 Same names, argument meaning, return values and implicit state (``cfgs.alpha``, the
-numpy global RNG) as the reference; the arithmetic runs on the B200 through libcpb200
+numpy global RNG) as the reference; the arithmetic runs on the H100 through libcpb200
 (see include/cpb200.h).  numpy in -> numpy out, exactly like the reference; torch CUDA
 tensors are accepted too and avoid the host<->device copies.
 

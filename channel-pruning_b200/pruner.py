@@ -1,4 +1,4 @@
-"""Layer-problem driver: one network's independent pruning problems on one or more B200s.
+"""Layer-problem driver: one network's independent pruning problems on one or more H100s.
 
 Within a GPU, problems are pipelined over the engine's streams in two phases (the only host
 synchronisation points): phase 1 enqueues gather -> Gram statistics -> LASSO search for every
@@ -131,21 +131,28 @@ def prune_layers(eng: Engine, shapes, datas, right0=1e-3, rank_tol=.1, from_host
     return [res_o[inv[i]] for i in range(len(shapes))]
 
 
-def _zero_copy_seconds(s):
-    """Model of the in-place gather over PCIe: it is bound by the number of read requests (one per 128-byte
-    line touched: the k rows of a window are W*4 bytes apart), ~4.5e8 lines/s measured (profiles/r1c_summary.md)."""
+# read requests per second of the in-place gather over PCIe (profiles/zc_rate.py; H100 80GB HBM3 SXM, PCIe 5)
+ZC_LINES_PER_S = 2.6e8
+
+
+def zero_copy_lines(s):
+    """128-byte lines the in-place gather touches in host memory (the k rows of a window are W*4 bytes apart)."""
     row = s.W * 4 if hasattr(s, "W") else 4 * 64
     lines = min(s.k, -(-((s.k - 1) * row + s.k * 4) // 128) + 1) if s.k > 1 else 1
-    return s.N * s.c * lines / 4.5e8
+    return s.N * s.c * lines
+
+
+def _zero_copy_seconds(s):
+    """Model of the in-place gather over PCIe: it is bound by the number of read requests."""
+    return zero_copy_lines(s) / ZC_LINES_PER_S
 
 
 def h2d_plan(shapes, datas, from_host):
     """Per layer: 'zc' (gather kernel reads the windows in place from pinned host memory) or 'dma' (copy engine
     moves the whole map at full PCIe bandwidth, gather from HBM).  DMA pays off when the windows cover most of
     the map (small spatial maps: conv5_x).  CPB200_DMA_MAX_MB caps the size of a map that may be staged.
-    Tried and measured worse (profiles/r2_summary.md): also staging one conv4_x map (802 MB) on the copy engine next to
-    the reader -- 86.1 instead of 78.7 ms per step; the two paths share the link (the reader slows down 1.7x while a
-    copy is in flight), so moving work between them buys nothing unless it removes bytes."""
+    The reader and the copy engine share the link, so moving a map from one to the other buys nothing unless it
+    removes bytes."""
     if from_host == "zc":
         return ["zc"] * len(shapes)
     if from_host == "copy":
@@ -244,10 +251,9 @@ def _prune_layers_ordered(eng, shapes, datas, right0, rank_tol, from_host, to_ho
     out = [None] * len(shapes)
     # phase 2 in COMPLETION order of the searches (which layer finishes first depends on sizes and, with
     # host-resident inputs, on the transfer order): poll the events, reconstruct whichever is ready.
-    # A reconstruction of a wide layer is ~390 kernel launches (~1.3 ms of host time inside libcpb200 calls, which
-    # release the GIL): issued from one thread, the five c = 512 layers of VGG-16 queued behind one another on the
-    # HOST (step timeline, call 23: the last one was not even issued until 7.5 ms after its search had finished).
-    # Worker threads issue them side by side; the engine's current (handle, stream) slot is thread-local.
+    # A reconstruction of a wide layer is hundreds of kernel launches (host time inside libcpb200 calls, which
+    # release the GIL): issued from one thread, the c = 512 layers of VGG-16 would queue behind one another on the
+    # HOST.  Worker threads issue them side by side; the engine's current (handle, stream) slot is thread-local.
     checks = []
 
     def reconstruct_layer(i):

@@ -1,5 +1,5 @@
 /*
- * cpb200 -- C ABI of the B200-native channel-pruning solver (libcpb200.so).
+ * cpb200 -- C ABI of the H100-native channel-pruning solver (libcpb200.so).
  *
  * The reference (ethanhe42/channel-pruning) has no FFI of its own for this path:
  * the hot path is Python calling numpy / scikit-learn / scipy (SURVEY.md 8b).  Each
@@ -52,12 +52,11 @@ enum { CP_F32 = 0, CP_F64 = 1 };
 /* arithmetic of cp_gram */
 enum {
     CP_GRAM_FP64 = 0,  /* fp32 inputs widened to fp64, DFMA accumulate (exact products) */
-    CP_GRAM_3XTF32 = 1 /* tensor cores (tcgen05), three products of a 22-bit hi/lo operand split, fp32 TMEM
-                          accumulation per 128-row run, fp64 reduction over the runs.  Since round 2 the split is
-                          into two fp16 halves of the shifted and power-of-two scaled data (kind::f16, the same
-                          split precision as tf32 at twice the rate; csrc/gram_tc2.cu); the name of the constant
-                          is kept for source compatibility.  CPB200_GRAM_TC=1 selects the first-generation
-                          kind::tf32 kernel (csrc/gram_tc.cu). */
+    CP_GRAM_3XTF32 = 1 /* tensor cores (wgmma), three products of a 22-bit hi/lo operand split, fp32 register
+                          accumulation per 64-row run, fp64 reduction over the runs.  The split is into two fp16
+                          halves of the shifted and power-of-two scaled data (the same split precision as tf32 at
+                          twice the rate; csrc/gram_tc2.cu); the name of the constant is kept for source
+                          compatibility. */
 };
 
 int cp_version(void);
@@ -71,7 +70,7 @@ int64_t cp_launch_count(void);
 /* bytes of scratch currently owned by the handle (diagnostics) */
 int64_t cp_workspace_bytes(cp_handle_t h);
 /* Diagnostics for the roofline of the tensor-core Gram kernel: with profiling enabled, cp_gram (mode CP_GRAM_3XTF32)
- * records CUDA events on its stream right before and after the tcgen05 GEMM launch; cp_gram_kernel_ms waits for the
+ * records CUDA events on its stream right before and after the tensor-core GEMM launch; cp_gram_kernel_ms waits for the
  * second event and returns the elapsed time of that launch alone (bench.py divides the algorithmic flops by it). */
 int cp_gram_profile(cp_handle_t h, int enable);
 /* Arithmetic of the bulk products inside the following cp_ls_solve / cp_ls_factor / cp_ls_resolve calls on this handle
@@ -250,9 +249,9 @@ int cp_ls_residual(cp_handle_t h, const float *X, int64_t N, int K, int64_t ldx,
 /*
  * The split-precision tensor-core product the solver uses for its bulk updates when cp_ls_tensor_cores is on
  * (csrc/gemm_tc.cu), exposed for tests and measurements: the fp64 matrix products inside LinearRegression.fit's
- * solve (lib/decompose.py:665-666), evaluated with 22 mantissa bits per operand entry on tcgen05.
+ * solve (lib/decompose.py:665-666), evaluated with 22 mantissa bits per operand entry on wgmma.
  *   C[m, nn] = alpha * sum_r A[m * lda + r] * B[nn * ldb + r] + beta * C[m * ldc + nn]      (fp64 in, fp64 out)
- * lower bit 0: only the 256 x 256 tiles with row tile >= column tile are touched (M >= Nn); bit 1: B is stored
+ * lower bit 0: only the 128 x 128 tiles with row tile >= column tile are touched (M >= Nn); bit 1: B is stored
  * reduction-major, b(nn, r) = B[r * ldb + nn] (the factor's block row in the backward substitution).  R <= 1024.
  */
 int cp_gemm_tc_split(cp_handle_t h, int M, int Nn, int R, double alpha, const double *A, int64_t lda, const double *B,

@@ -1,6 +1,6 @@
 // Microbenchmark: latency of dependent fp64 operations on one warp (clock64 around an unrolled dependent chain),
 // the numbers that bound the serial recurrence of the LASSO coordinate descent (lasso.cu) and the pivot chain of
-// the Cholesky panel (ls.cu).   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o dp_latency dp_latency.cu
+// the Cholesky panel (ls.cu).   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o dp_latency dp_latency.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 

@@ -1,8 +1,8 @@
-// Round-2 microbenchmark: what does one intra-CTA hand-shake hop cost on sm_100a?
+// Microbenchmark: what does one intra-CTA hand-shake hop cost on sm_90a?
 //
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o mbar_hop profiles/mbar_hop.cu && ./mbar_hop
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o profiles/mbar_hop profiles/mbar_hop.cu && profiles/mbar_hop
 //
-// One CTA, NW "worker" warps and one single-thread "issuer" (the shape of gram_tc_kernel's converter <-> MMA ring).
+// One CTA, NW "worker" warps and one single-thread "issuer" (the shape of a producer <-> consumer stage ring).
 // Per round: every worker warp signals the issuer (fan-in), the issuer answers (fan-out); ROUNDS rounds, clock64
 // around the loop, result = cycles per round (= two hops).  DEPTH > 1 lets the workers run ahead by DEPTH rounds
 // (a ring of DEPTH barriers), which is what a multi-stage pipeline relies on to hide the hop latency.

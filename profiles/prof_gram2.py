@@ -1,6 +1,5 @@
-"""Second-generation tensor-core Gram (gram_tc2.cu) against an fp64 evaluation and against the first generation.
+"""Tensor-core Gram (gram_tc2.cu) against an fp64 evaluation.
     python profiles/prof_gram2.py            # accuracy on edge shapes + timing on the conv4_2 shape
-    CPB200_GRAM_TC=1 python profiles/prof_gram2.py   # the same with the first-generation kernel
 Timing: CUDA events around one cp_gram call (all its launches), L2 flushed between repetitions."""
 import os
 import sys
@@ -13,7 +12,6 @@ import cpb200
 
 eng = cpb200.Engine(gram_mode=1)
 dev = eng.device
-gen = "gen1" if os.environ.get("CPB200_GRAM_TC", "") == "1" else ("gen2-single" if os.environ.get("CPB200_GRAM_PAIR", "") == "0" else "gen2-pair")
 
 
 def check(N, K, n, seed=0, scale=1.0, offset=0.0):
@@ -38,8 +36,8 @@ def check(N, K, n, seed=0, scale=1.0, offset=0.0):
     ec = ((Gc - Gc_ref).abs() / torch.outer(dc, dc)).max().item()
     sym = bool((out["G"] == out["G"].T).all().item())
     esx = ((out["sx"] - X64.sum(0)).abs() / X64.sum(0).abs().clamp_min(1e-30)).max().item()
-    print("%s N=%6d K=%5d n=%4d scale=%g off=%g: relG %.2e relB %.2e centred %.2e sx %.1e sym %s" %
-          (gen, N, K, n, scale, offset, eg, eb, ec, esx, sym), flush=True)
+    print("N=%6d K=%5d n=%4d scale=%g off=%g: relG %.2e relB %.2e centred %.2e sx %.1e sym %s" %
+          (N, K, n, scale, offset, eg, eb, ec, esx, sym), flush=True)
     return max(eg, eb, ec)
 
 
@@ -56,8 +54,7 @@ d = cpb200.synth.make_problem_device(s, 5, eng, layout="nhwc")
 X = eng.patch_gather(d["fmap"], d["randx"], d["randy"], s.B, s.P, s.k, s.pad, s.stride, relu=True, layout="nhwc")
 flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
 ts, tk = [], []
-if gen != "gen1":
-    eng.gram_profile(True)
+eng.gram_profile(True)
 for it in range(8):
     flush.fill_(it)
     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -66,14 +63,12 @@ for it in range(8):
     b.record()
     torch.cuda.synchronize()
     ts.append(a.elapsed_time(b))
-    if gen != "gen1":
-        tk.append(eng.gram_kernel_ms())
+    tk.append(eng.gram_kernel_ms())
 flop = s.N * s.K * (s.K + 1) + 2.0 * s.N * s.K * s.n
-print("%s cp_gram conv4_2 N=%d: %s ms -> best %.4f ms = %.1f TF/s algorithmic" %
-      (gen, s.N, ["%.3f" % t for t in ts], min(ts[2:]), flop / (min(ts[2:]) / 1e3) / 1e12), flush=True)
-if tk:
-    print("%s GEMM kernel alone: %s ms -> best %.4f ms = %.1f TF/s algorithmic (x3 issued)" %
-          (gen, ["%.3f" % t for t in tk], min(tk[2:]), flop / (min(tk[2:]) / 1e3) / 1e12), flush=True)
+print("cp_gram conv4_2 N=%d: %s ms -> best %.4f ms = %.1f TF/s algorithmic" %
+      (s.N, ["%.3f" % t for t in ts], min(ts[2:]), flop / (min(ts[2:]) / 1e3) / 1e12), flush=True)
+print("GEMM kernel alone: %s ms -> best %.4f ms = %.1f TF/s algorithmic (x3 issued)" %
+      (["%.3f" % t for t in tk], min(tk[2:]), flop / (min(tk[2:]) / 1e3) / 1e12), flush=True)
 X64 = X.double()
 Gr = X64.T @ X64
 dx = Gr.diagonal().sqrt()

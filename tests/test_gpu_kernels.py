@@ -312,9 +312,9 @@ def test_rank_deficient_system_gets_gelsd_truncated_solution(engine, mode):
 def test_gemm_tc_split_matches_fp64(engine, M, Nn, R, lower):
     """cp_gemm_tc_split (the solver's tensor-core bulk product): C = beta C + alpha A B', rows of very different magnitude
     (power-of-two row scales).  Tolerance: |err| <= 4e-6 * sum_r |a||b|.  The operand split keeps 22 bits (<= 5e-7 of
-    sum|a||b|); the rest is the tensor core's fp32 accumulator, which TRUNCATES: up to 24 (R <= 256) or 48 additions
-    per accumulator, each losing < 2^-23 of the running sum in the same direction when all terms have one sign -- the
-    diagonal of a symmetric update (measured: 1.5e-6 there, 3.5e-7 for mixed signs)."""
+    sum|a||b|); the rest is the tensor core's fp32 accumulator, which TRUNCATES: 12 additions per accumulator
+    run (64 reduction elements), each losing < 2^-23 of the running sum in the same direction when all terms have one sign -- the
+    diagonal of a symmetric update, the worst case (mixed signs partly cancel)."""
     r = np.random.RandomState(M + Nn + R)
     A = r.standard_normal((M, R)) * np.exp(3.0 * r.standard_normal((M, 1)))
     if lower is True:
@@ -330,8 +330,8 @@ def test_gemm_tc_split_matches_fp64(engine, M, Nn, R, lower):
     ref = C0 - A @ B.T
     bound = np.abs(A) @ np.abs(B).T
     err = np.abs(got - ref) / bound
-    if lower:  # 256 x 256 tiles with row tile >= column tile are written; the others must be untouched
-        ti, tj = np.arange(M)[:, None] // 256, np.arange(Nn)[None, :] // 256
+    if lower:  # 128 x 128 tiles with row tile >= column tile are written; the others must be untouched
+        ti, tj = np.arange(M)[:, None] // 128, np.arange(Nn)[None, :] // 128
         touched = ti >= tj
         assert np.array_equal(got[~touched], C0[~touched])
         err = err[touched]

@@ -109,8 +109,8 @@ def test_r3_stage_by_stage_against_reference_golden(engine, golden_dir, name, mo
 def test_r3_free_running_walk(engine, golden_dir, name, mode):
     """The same walk left alone.  The blobs behind an approximated layer are nearly rank deficient (sigma_min/sigma_max
     of the conv2_2 patches here: 1e-3), so the pseudo-inverses of the next stage amplify the differences of the
-    previous one by about that ratio (measured: 1e-7 -> 3.5e-5 with exact-product statistics, 3e-6 -> 1e-2 with the
-    tensor-core ones; the stage-by-stage test above bounds each stage's own deviation at 3e-6 in both).  Individual
+    previous one by about that ratio (the stage-by-stage test above bounds each stage's own deviation at 3e-6 in both
+    modes).  Individual
     weights are therefore compared loosely; what must hold is what the reference guarantees -- the discrete outcome
     (selections, alpha schedule, RNG draws) and the function the network computes."""
     from cpb200.lib import cfgs
