@@ -13,11 +13,8 @@
 // reference takes SVDs of on this path is small (VH: (c k) x (n k) <= 1536 x 1536; ITQ: reduced to n x n, n <= 512,
 // because X = G M has the right singular vectors of the n x n matrix L_S' M with G'G = L_S L_S') so the kernel keeps
 // both columns of a pair in shared memory.  Jacobi is also the most accurate dense SVD (high relative accuracy).
-#include <cstdlib>
-
 #include "common.cuh"
 #include "gemm_f64.cuh"
-#include "gemm_async.cuh"
 
 namespace {
 
@@ -47,7 +44,7 @@ int gemm_any(cp_handle_t h, const double *A, int64_t lda, const double *B, int64
     g.tile_mode = TILES_ALL;
     g.a_vec = al16d(A) && (lda % 2 == 0);
     g.b_vec = al16d(B) && (ldb % 2 == 0);
-    const int tiles = num_tiles(M, Nn, TILES_ALL);
+    const int tiles = num_tiles(M, Nn, TILES_ALL, BM);
     const int target = 2 * h->num_sms;
     int nsplit = 1;
     if (tiles < target && R >= 8 * BK) {  // tall-skinny products: split the reduction over CTAs
@@ -60,22 +57,11 @@ int gemm_any(cp_handle_t h, const double *A, int64_t lda, const double *B, int64
     rps = (rps + BK - 1) / BK * BK;
     nsplit = (int)((R + rps - 1) / rps);
     if (nsplit <= 1) {
-        if constexpr (!A_MC) {  // plain fp64 operands: the cp.async-staged kernel (gemm_async.cuh)
-            cpasync::Args a{};
-            a.A = A; a.lda = lda; a.B = B; a.ldb = ldb; a.C = C; a.ldc = ldc;
-            a.M = M; a.Nn = Nn; a.R = (int)R;
-            a.alpha = alpha; a.beta = beta; a.tile_mode = cpasync::TILES_ALL;
-            static const bool on = [] { const char *e = getenv("CPB200_GEMM"); return !e || e[0] == 'a' || e[0] == 'A'; }();
-            if (on && R > 0 && R <= 0x7fffffff && cpasync::eligible(a)) {
-                if (tiles >= h->num_sms) CP_GEMM_LAUNCH((cpasync::launch<128, B_NC>(a, stream)));
-                else CP_GEMM_LAUNCH((cpasync::launch<64, B_NC>(a, stream)));
-                return CP_OK;
-            }
-        }
         g.nsplit = 1;
         g.r_per_split = R > 0 ? R : 1;
         g.C = C; g.ldc = ldc;
-        CP_GEMM_LAUNCH((launch<double, double, A_MC, B_NC>(g, stream)));
+        // fewer 128 x 128 tiles than SMs: 64 x 64 tiles if the cp.async kernel takes the product
+        CP_GEMM_LAUNCH((launch<double, double, A_MC, B_NC>(g, stream, tiles >= h->num_sms ? 128 : 64)));
         return CP_OK;
     }
     void *ws = nullptr;

@@ -21,7 +21,6 @@
 // Bound: the read-modify-write of C (16 bytes per 2R flop) for R <= 512, then the tensor pipe.
 #include <cuda.h>
 #include <cuda_fp16.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 #include "tc_common.cuh"
@@ -198,11 +197,6 @@ gemm_tc_prep_t(const double *__restrict__ P, int64_t ld, int ncols, int R, int R
 }
 
 }  // namespace
-
-bool cp_gemm_tc_enabled() {
-    static const bool on = [] { const char *e = getenv("CPB200_LS_TC"); return !(e && e[0] == '0'); }();
-    return on;
-}
 
 // slot: which of the handle's operand buffers to use -- one per stream the solver issues work on (calls on one stream
 // are ordered, so a buffer is never rewritten under a kernel that still reads it)

@@ -3,7 +3,7 @@
 // Replaces the O(N K^2) passes of LinearRegression.fit (reference lib/decompose.py:665-666)
 // and of the LASSO design matrix (lib/decompose.py:428-434,457); see SURVEY.md 7.1.
 //
-// CP_GRAM_FP64: fp32 inputs widened to fp64 in registers, DFMA accumulation
+// CP_GRAM_FP64: fp32 inputs widened to fp64 in registers, fp64 accumulation on DMMA
 // (cpgemm::gemm_kernel).  Every product of two fp32 values is exact in fp64, so the
 // only rounding is the fp64 accumulation -- the same arithmetic class as the
 // reference's float64 numpy path.  Small K does not fill the SMs with output tiles,
@@ -113,7 +113,7 @@ static int gram_product(cp_handle_t h, const float *A, int64_t lda, int M, const
     g.tile_mode = sym ? TILES_UPPER_SYM : TILES_ALL;
     g.a_vec = aligned16(A) && (lda % 4 == 0);
     g.b_vec = aligned16(B) && (ldb % (16 / sizeof(TB)) == 0);
-    const int tiles = num_tiles(M, Nn, g.tile_mode);
+    const int tiles = num_tiles(M, Nn, g.tile_mode, BM);
     const int target = 2 * h->num_sms;
     int nsplit = 1;
     if (tiles < target) {

@@ -23,14 +23,9 @@
 // reads and writes the same tile, whatever the tile shape.
 // Bound: the dependency chain of ~K'/128 x (potrf128 + 2 small GEMMs) for the factorisation,
 // the FP64 pipe for the far updates (K'^3/3 flop).
-#include <cstdlib>
-
 #include "common.cuh"
 #include "gemm_f64.cuh"
-#include "gemm_small.cuh"
-#include "gemm_async.cuh"
 
-bool cp_gemm_tc_enabled();
 int cp_gemm_tc_f64(cp_handle_t h, int slot, const double *A, int64_t lda, const double *B, int64_t ldb, double *C,
                    int64_t ldc, int M, int Nn, int R, double alpha, double beta, int lower, cudaStream_t stream,
                    int max_ctas, int b_nc);
@@ -444,93 +439,34 @@ ls_output(const double *__restrict__ Wt, int64_t ld, const double *__restrict__ 
 
 inline bool al16(const void *p) { return ((uintptr_t)p & 15) == 0; }
 
-// CPB200_GEMM: "async" (default: cp.async-staged DMMA kernels of gemm_async.cuh for the solver's fp64 products),
-// "dmma" / "dfma" (register-staged kernels of gemm_f64.cuh / gemm_small.cuh with the MMA or the FMA inner loop)
-bool use_async_gemm() {
-    static const bool on = [] {
-        const char *e = getenv("CPB200_GEMM");
-        return !e || e[0] == 'a' || e[0] == 'A';
-    }();
-    return on;
-}
-template <int T, bool B_NC>
-int dgemm_async(const double *A, int64_t lda, const double *B, int64_t ldb, double *C, int64_t ldc, int M, int Nn, int64_t R,
-                double alpha, double beta, int tile_mode, cudaStream_t stream, int max_ctas, bool *done) {
-    cpasync::Args g{};
-    g.A = A; g.lda = lda; g.B = B; g.ldb = ldb; g.C = C; g.ldc = ldc;
-    g.M = M; g.Nn = Nn; g.R = (int)R;
-    g.alpha = alpha; g.beta = beta; g.tile_mode = tile_mode; g.max_ctas = max_ctas;
-    *done = false;
-    if (!use_async_gemm() || !cpasync::eligible(g) || R > 0x7fffffff) return CP_OK;
-    *done = true;
-    if (M <= 0 || Nn <= 0) return CP_OK;
-    CP_GEMM_LAUNCH((cpasync::launch<T, B_NC>(g, stream)));
-    return CP_OK;
-}
-
-// 128 x 128 tiles (throughput: the far trailing updates)
-int dgemm_big(const double *A, int64_t lda, const double *B, int64_t ldb, double *C, int64_t ldc, int M, int Nn,
-              int64_t R, double alpha, double beta, int tile_mode, cudaStream_t stream, int max_ctas = 0,
-              cp_handle_t tc = nullptr) {
-    using namespace cpgemm;
-    // tensor-core handle given and enabled: split-precision product (gemm_tc.cu) for everything wide enough to fill
-    // its 128 x 128 tiles; one operand buffer per stream of the solver
-    static const int tc_min_nn = [] { const char *e = getenv("CPB200_LS_TC_MIN_NN"); return e ? atoi(e) : 192; }();
-    if (tc && tc->ls_tc && cp_gemm_tc_enabled() && R >= 128 && R <= 1024 && Nn >= tc_min_nn && M >= 256 &&
-        (tile_mode == TILES_ALL || tile_mode == TILES_LOWER)) {
-        const int slot = stream == tc->side ? 1 : (stream == tc->bulk ? 2 : 0);
-        return cp_gemm_tc_f64(tc, slot, A, lda, B, ldb, C, ldc, M, Nn, (int)R, alpha, beta, tile_mode == TILES_LOWER, stream,
-                              max_ctas, 0);
-    }
-    bool done = false;
-    int rca = dgemm_async<128, false>(A, lda, B, ldb, C, ldc, M, Nn, R, alpha, beta, tile_mode, stream, max_ctas, &done);
-    if (rca || done) return rca;
-    Args g{};
-    g.A = A; g.lda = lda; g.B = B; g.ldb = ldb; g.C = C; g.ldc = ldc;
-    g.M = M; g.Nn = Nn; g.R = R;
-    g.nsplit = 1; g.r_per_split = R;
-    g.alpha = alpha; g.beta = beta; g.tile_mode = tile_mode;
-    g.a_vec = al16(A) && (lda % 2 == 0);
-    g.b_vec = al16(B) && (ldb % 2 == 0);
-    g.max_ctas = max_ctas;
-    if (M <= 0 || Nn <= 0) return CP_OK;
-    CP_GEMM_LAUNCH((launch<double, double, false, false>(g, stream)));
-    return CP_OK;
-}
-// 64 x 64 tiles (latency: everything on the dependency chain)
+// C = alpha * a b' + beta C on the solver's fp64 operands:  a(m, r) = A[m * lda + r],
+// b(nn, r) = B_NC ? B[r * ldb + nn] : B[nn * ldb + r].
+// tc: the product may take the tensor cores.  With the handle's tensor-core mode on, products wide enough to fill the
+// 128 x 128 tiles of the split-precision kernel (gemm_tc.cu) run there, on one operand buffer per stream of the solver.
+// Everything else runs on gemm_async_kernel with tile x tile tiles (128: throughput; 64: latency, everything on the
+// dependency chain).  The operands never need the register-staged kernel: every matrix here is carved 256-byte aligned
+// (cp_carver, h->fac), every leading dimension is ld_for(K) or GB, and every column offset a multiple of 128.
 template <bool B_NC>
-int dgemm_small(const double *A, int64_t lda, const double *B, int64_t ldb, double *C, int64_t ldc, int M, int Nn,
-                int R, double alpha, double beta, int tile_mode, cudaStream_t stream) {
-    using namespace cpsmall;
-    bool done = false;
-    int rca = dgemm_async<64, B_NC>(A, lda, B, ldb, C, ldc, M, Nn, R, alpha, beta, tile_mode, stream, 0, &done);
-    if (rca || done) return rca;
-    Args g{};
-    g.A = A; g.lda = lda; g.B = B; g.ldb = ldb; g.C = C; g.ldc = ldc;
-    g.M = M; g.Nn = Nn; g.R = R;
-    g.alpha = alpha; g.beta = beta; g.tile_mode = tile_mode;
-    g.a_vec = al16(A) && (lda % 2 == 0);
-    g.b_vec = al16(B) && (ldb % 2 == 0);
+int dgemm(cp_handle_t h, bool tc, int tile, int tile_mode, int max_ctas, const double *A, int64_t lda, const double *B,
+          int64_t ldb, double *C, int64_t ldc, int M, int Nn, int R, double alpha, double beta, cudaStream_t stream) {
+    using namespace cpgemm;
+    if (tc && h->ls_tc && R >= 128 && R <= 1024 && Nn >= 192 && M >= 256 &&
+        (tile_mode == TILES_ALL || tile_mode == TILES_LOWER)) {
+        const int slot = stream == h->side ? 1 : (stream == h->bulk ? 2 : 0);
+        return cp_gemm_tc_f64(h, slot, A, lda, B, ldb, C, ldc, M, Nn, R, alpha, beta, tile_mode == TILES_LOWER, stream,
+                              max_ctas, B_NC);
+    }
+    const AsyncArgs g{A, lda, B, ldb, C, ldc, M, Nn, R, alpha, beta, tile_mode, max_ctas};
+    CP_REQUIRE(aligned(g), "least-squares GEMM: operand not 16-byte aligned (A %p lda %lld, B %p ldb %lld)", (const void *)A,
+               (long long)lda, (const void *)B, (long long)ldb);
     if (M <= 0 || Nn <= 0) return CP_OK;
-    CP_GEMM_LAUNCH((launch<B_NC>(g, stream)));
+    if (tile == 128) CP_GEMM_LAUNCH((launch_async<128, B_NC>(g, stream)));
+    else CP_GEMM_LAUNCH((launch_async<64, B_NC>(g, stream)));
     return CP_OK;
 }
 
 // The look-ahead stream runs one priority level below the stream of the first solve on this handle (a handle serves one
 // stream in the layer pipeline): behind its own chain, ahead of cheaper problems' work.
-// grid cap of the bulk trailing updates: two thirds of the SMs (CPB200_LS_REST_CTAS overrides; 0 = uncapped)
-int device_sms() {  // SMs of the current device
-    int d = 0, n = 0;
-    cudaGetDevice(&d);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, d);
-    return n;
-}
-
-int rest_ctas(cp_handle_t h) {
-    static const int env = [] { const char *e = getenv("CPB200_LS_REST_CTAS"); return e ? atoi(e) : -1; }();
-    return env >= 0 ? env : h->num_sms * 2 / 3;
-}
-
 int ensure_side(cp_handle_t h, cudaStream_t stream) {
     if (!h->side) {
         int lo = 0, hi = 0, p = 0;
@@ -559,43 +495,23 @@ int configure_potrf(cp_handle_t h) {
 
 }  // namespace
 
-// dense product on 128 x 128 tiles with the (m, r) x (r, nn) operand layout of the substitutions
-static int dgemm_big_nc(const double *A, int64_t lda, const double *B, int64_t ldb, double *C, int64_t ldc, int M, int Nn,
-                        int64_t R, double alpha, double beta, cudaStream_t stream, cp_handle_t tc = nullptr) {
-    using namespace cpgemm;
-    if (tc && tc->ls_tc && cp_gemm_tc_enabled() && R >= 128 && R <= 1024 && Nn >= 192 && M >= 256) {
-        const int slot = stream == tc->side ? 1 : (stream == tc->bulk ? 2 : 0);
-        return cp_gemm_tc_f64(tc, slot, A, lda, B, ldb, C, ldc, M, Nn, (int)R, alpha, beta, 0, stream, 0, 1);
-    }
-    bool done = false;
-    int rca = dgemm_async<128, true>(A, lda, B, ldb, C, ldc, M, Nn, R, alpha, beta, cpasync::TILES_ALL, stream, 0, &done);
-    if (rca || done) return rca;
-    Args g{};
-    g.A = A; g.lda = lda; g.B = B; g.ldb = ldb; g.C = C; g.ldc = ldc;
-    g.M = M; g.Nn = Nn; g.R = R;
-    g.nsplit = 1; g.r_per_split = R;
-    g.alpha = alpha; g.beta = beta; g.tile_mode = TILES_ALL;
-    g.a_vec = al16(A) && (lda % 2 == 0);
-    g.b_vec = al16(B) && (ldb % 2 == 0);
-    if (M <= 0 || Nn <= 0) return CP_OK;
-    CP_GEMM_LAUNCH((launch<double, double, false, true>(g, stream)));
-    return CP_OK;
-}
-
 static inline int ngroups(int Kd) { return (Kd + GB - 1) / GB; }
 static inline size_t xinv_elems(int Kd) { return (size_t)ngroups(Kd) * GB * GB; }
 
 // X21 = -X22 * L21 * X11 inside one group block X (GB x GB, leading dimension GB): rows/cols [a0, a1) and [a1, a2)
 // of the group hold the already inverted diagonal parts X11 and X22; L21 = the factor's rows a1..a2, columns a0..a1.
-static int merge_inverse(double *X, const double *L21, int64_t ld, int a0, int a1, int a2, double *T, cudaStream_t stream) {
+static int merge_inverse(cp_handle_t h, double *X, const double *L21, int64_t ld, int a0, int a1, int a2, double *T,
+                         cudaStream_t stream) {
+    using namespace cpgemm;
     const int h1 = a1 - a0, h2 = a2 - a1;
     if (h1 <= 0 || h2 <= 0) return CP_OK;
     // T = L21 * X11        (h2 x h1, inner h1)
-    int rc = dgemm_small<true>(L21, ld, X + (int64_t)a0 * GB + a0, GB, T, GB, h2, h1, h1, 1.0, 0.0, cpsmall::TILES_ALL, stream);
+    int rc = dgemm<true>(h, false, 64, TILES_ALL, 0, L21, ld, X + (int64_t)a0 * GB + a0, GB, T, GB, h2, h1, h1, 1.0, 0.0,
+                         stream);
     if (rc) return rc;
     // X21 = -X22 * T       (h2 x h1, inner h2)
-    return dgemm_small<true>(X + (int64_t)a1 * GB + a1, GB, T, GB, X + (int64_t)a1 * GB + a0, GB, h2, h1, h2, -1.0, 0.0,
-                             cpsmall::TILES_ALL, stream);
+    return dgemm<true>(h, false, 64, TILES_ALL, 0, X + (int64_t)a1 * GB + a1, GB, T, GB, X + (int64_t)a1 * GB + a0, GB, h2,
+                       h1, h2, -1.0, 0.0, stream);
 }
 
 // Factorisation.  M: (Kd + nrhs) x Kd (leading dimension ld): rows 0..Kd-1 an SPD matrix (lower part used, destroyed),
@@ -640,8 +556,8 @@ static int chol_factor(cp_handle_t h, double *M, double *L, int64_t ld, int Kd, 
         const int below = Ktot - j1;
         if (below > 0) {
             // block column of the factor: rows below * L_d^-T  (right-hand-side rows included)
-            rc = dgemm_small<false>(M + (int64_t)j1 * ld + j0, ld, Lp, GB, L + (int64_t)j1 * ld + j0, ld, below, nb, nb, 1.0,
-                                    0.0, cpsmall::TILES_ALL, stream);
+            rc = dgemm<false>(h, false, 64, TILES_ALL, 0, M + (int64_t)j1 * ld + j0, ld, Lp, GB, L + (int64_t)j1 * ld + j0,
+                              ld, below, nb, nb, 1.0, 0.0, stream);
             if (rc) return rc;
         }
         const int ncols = Kd - j1;
@@ -658,11 +574,11 @@ static int chol_factor(cp_handle_t h, double *M, double *L, int64_t ld, int Kd, 
             const int ge = (j1 - g0);  // columns of the group factored so far
             if (og & 1) {              // pair (og-1, og): [a0, a0+128) and [a0+128, ge)
                 const int a0 = (og - 1) * PB;
-                rc = merge_inverse(Xg, L + (int64_t)(g0 + a0 + PB) * ld + g0 + a0, ld, a0, a0 + PB, ge, Tg, h->side);
+                rc = merge_inverse(h, Xg, L + (int64_t)(g0 + a0 + PB) * ld + g0 + a0, ld, a0, a0 + PB, ge, Tg, h->side);
                 if (rc) return rc;
             }
             if (last_in_group && ge > 2 * PB) {  // halves [0, 256) and [256, ge)
-                rc = merge_inverse(Xg, L + (int64_t)(g0 + 2 * PB) * ld + g0, ld, 0, 2 * PB, ge, Tg, h->side);
+                rc = merge_inverse(h, Xg, L + (int64_t)(g0 + 2 * PB) * ld + g0, ld, 0, 2 * PB, ge, Tg, h->side);
                 if (rc) return rc;
             }
         }
@@ -673,15 +589,16 @@ static int chol_factor(cp_handle_t h, double *M, double *L, int64_t ld, int Kd, 
             side_pending = false;
         }
         const double *Pn = L + (int64_t)j1 * ld + j0;
-        rc = dgemm_small<false>(Pn, ld, Pn, ld, M + (int64_t)j1 * ld + j1, ld, Ktot - j1, w2, nb, -1.0, 1.0,
-                                cpsmall::TILES_LOWER, stream);
+        rc = dgemm<false>(h, false, 64, TILES_LOWER, 0, Pn, ld, Pn, ld, M + (int64_t)j1 * ld + j1, ld, Ktot - j1, w2, nb,
+                          -1.0, 1.0, stream);
         if (rc) return rc;
         if (!more) continue;
         const int j2 = j1 + w2;
         if (!odd) {
             const int w3 = Kd - j2 < PB ? Kd - j2 : PB;
             const double *Pf = L + (int64_t)j2 * ld + j0;
-            rc = dgemm_big(Pf, ld, Pf, ld, M + (int64_t)j2 * ld + j2, ld, Ktot - j2, w3, nb, -1.0, 1.0, TILES_LOWER, h->side, 0, h);
+            rc = dgemm<false>(h, true, 128, TILES_LOWER, 0, Pf, ld, Pf, ld, M + (int64_t)j2 * ld + j2, ld, Ktot - j2, w3, nb,
+                              -1.0, 1.0, h->side);
             if (rc) return rc;
             CP_CUDA(cudaEventRecord(h->ev_side, h->side));
             side_pending = true;
@@ -690,7 +607,8 @@ static int chol_factor(cp_handle_t h, double *M, double *L, int64_t ld, int Kd, 
             const int je = j0 - PB, R2 = PB + nb;
             const int wn = Kd - j2 < 2 * PB ? Kd - j2 : 2 * PB;  // near: the next pair's two block columns
             const double *Pq = L + (int64_t)j2 * ld + je;
-            rc = dgemm_big(Pq, ld, Pq, ld, M + (int64_t)j2 * ld + j2, ld, Ktot - j2, wn, R2, -1.0, 1.0, TILES_LOWER, h->side, 0, h);
+            rc = dgemm<false>(h, true, 128, TILES_LOWER, 0, Pq, ld, Pq, ld, M + (int64_t)j2 * ld + j2, ld, Ktot - j2, wn, R2,
+                              -1.0, 1.0, h->side);
             if (rc) return rc;
             CP_CUDA(cudaEventRecord(h->ev_side, h->side));
             side_pending = true;
@@ -702,16 +620,17 @@ static int chol_factor(cp_handle_t h, double *M, double *L, int64_t ld, int Kd, 
                 }
                 const int wm = Kd - j4 < 2 * PB ? Kd - j4 : 2 * PB;
                 const double *P4 = L + (int64_t)j4 * ld + je;
-                rc = dgemm_big(P4, ld, P4, ld, M + (int64_t)j4 * ld + j4, ld, Ktot - j4, wm, R2, -1.0, 1.0, TILES_LOWER, h->side, 0, h);
+                rc = dgemm<false>(h, true, 128, TILES_LOWER, 0, P4, ld, P4, ld, M + (int64_t)j4 * ld + j4, ld, Ktot - j4, wm,
+                                  R2, -1.0, 1.0, h->side);
                 if (rc) return rc;
                 const int j6 = j4 + wm;
                 if (Kd - j6 > 0) {
                     // the bulk of the trailing update has slack; its long-running tiles must not take every SM either,
-                    // or the chain's small kernels queue behind them
+                    // or the chain's small kernels queue behind them: two thirds of the SMs
                     CP_CUDA(cudaStreamWaitEvent(h->bulk, h->ev_panel, 0));
                     const double *Pr = L + (int64_t)j6 * ld + je;
-                    rc = dgemm_big(Pr, ld, Pr, ld, M + (int64_t)j6 * ld + j6, ld, Ktot - j6, Kd - j6, R2, -1.0, 1.0,
-                                   TILES_LOWER, h->bulk, rest_ctas(h), h);
+                    rc = dgemm<false>(h, true, 128, TILES_LOWER, h->num_sms * 2 / 3, Pr, ld, Pr, ld, M + (int64_t)j6 * ld + j6,
+                                      ld, Ktot - j6, Kd - j6, R2, -1.0, 1.0, h->bulk);
                     if (rc) return rc;
                     CP_CUDA(cudaEventRecord(h->ev_bulk, h->bulk));
                     bulk_pending = true;
@@ -729,25 +648,23 @@ static int chol_factor(cp_handle_t h, double *M, double *L, int64_t ld, int Kd, 
 }
 
 // Forward substitution of further right-hand sides: Zt (n x Kd, ld) is destroyed, F (n x Kd, ld) receives (L^-1 Rhs)'.
-static int chol_forward(const double *L, int64_t ld, int Kd, const double *Xinv, double *Zt, double *F, int64_t ldz, int n,
-                        cudaStream_t stream, cp_handle_t tc = nullptr) {
+static int chol_forward(cp_handle_t h, const double *L, int64_t ld, int Kd, const double *Xinv, double *Zt, double *F,
+                        int64_t ldz, int n, cudaStream_t stream) {
+    using namespace cpgemm;
     for (int g0 = 0; g0 < Kd; g0 += GB) {
         const int gs = Kd - g0 < GB ? Kd - g0 : GB;
         const int g1 = g0 + gs;
         const double *Xg = Xinv + (size_t)(g0 / GB) * GB * GB;
         // F_g = Zt_g * Xinv_g'   (C[t, i] = sum_r Zt[t, g0 + r] * Xinv_g[i, r])
-        int rc = dgemm_small<false>(Zt + g0, ldz, Xg, GB, F + g0, ldz, n, gs, gs, 1.0, 0.0, cpsmall::TILES_ALL, stream);
+        int rc = dgemm<false>(h, false, 64, TILES_ALL, 0, Zt + g0, ldz, Xg, GB, F + g0, ldz, n, gs, gs, 1.0, 0.0, stream);
         if (rc) return rc;
         if (Kd - g1 > 0) {  // Zt[:, g1:] -= F_g * L[g1:, g0:g1]'
             // few right-hand sides: 128 x 128 tiles would leave most SMs idle on a 512-deep product, 64 x 64 tiles fill them
             // tensor-core mode: split-precision tiles (n >= 256 right-hand sides, a few column tiles) beat the fp64 pipe
-            const bool use_tc = tc && tc->ls_tc && cp_gemm_tc_enabled() && n >= 256 && Kd - g1 >= 512;
-            if (use_tc || cpgemm::num_tiles(n, Kd - g1, cpgemm::TILES_ALL) >= 2 * device_sms())
-                rc = dgemm_big(F + g0, ldz, L + (int64_t)g1 * ld + g0, ld, Zt + g1, ldz, n, Kd - g1, gs, -1.0, 1.0,
-                               cpgemm::TILES_ALL, stream, 0, use_tc ? tc : nullptr);
-            else
-                rc = dgemm_small<false>(F + g0, ldz, L + (int64_t)g1 * ld + g0, ld, Zt + g1, ldz, n, Kd - g1, gs, -1.0, 1.0,
-                                        cpsmall::TILES_ALL, stream);
+            const bool use_tc = h->ls_tc && n >= 256 && Kd - g1 >= 512;
+            const int tile = use_tc || num_tiles(n, Kd - g1, TILES_ALL, BM) >= 2 * h->num_sms ? 128 : 64;
+            rc = dgemm<false>(h, use_tc, tile, TILES_ALL, 0, F + g0, ldz, L + (int64_t)g1 * ld + g0, ld, Zt + g1, ldz, n,
+                              Kd - g1, gs, -1.0, 1.0, stream);
             if (rc) return rc;
         }
     }
@@ -755,23 +672,22 @@ static int chol_forward(const double *L, int64_t ld, int Kd, const double *Xinv,
 }
 
 // Backward substitution: F (n x Kd, ldf; destroyed) holds (L^-1 Rhs)'; Wt (n x Kd, ldw) receives (SPD^-1 Rhs)'.
-static int chol_backward(const double *L, int64_t ld, int Kd, const double *Xinv, double *F, int64_t ldf, double *Wt,
-                         int64_t ldw, int n, cudaStream_t stream, cp_handle_t tc = nullptr) {
+// tc: the bulk products may take the tensor cores (not in the dual path, whatever the handle's mode).
+static int chol_backward(cp_handle_t h, bool tc, const double *L, int64_t ld, int Kd, const double *Xinv, double *F,
+                         int64_t ldf, double *Wt, int64_t ldw, int n, cudaStream_t stream) {
+    using namespace cpgemm;
     for (int g = ngroups(Kd) - 1; g >= 0; --g) {
         const int g0 = g * GB;
         const int gs = Kd - g0 < GB ? Kd - g0 : GB;
         const double *Xg = Xinv + (size_t)g * GB * GB;
         // Wt_g = F_g * Xinv_g   (C[t, i] = sum_r F[t, g0 + r] * Xinv_g[r, i])
-        int rc = dgemm_small<true>(F + g0, ldf, Xg, GB, Wt + g0, ldw, n, gs, gs, 1.0, 0.0, cpsmall::TILES_ALL, stream);
+        int rc = dgemm<true>(h, false, 64, TILES_ALL, 0, F + g0, ldf, Xg, GB, Wt + g0, ldw, n, gs, gs, 1.0, 0.0, stream);
         if (rc) return rc;
         if (g0 > 0) {  // F[:, 0:g0] -= Wt_g * L[g0:g0+gs, 0:g0]
-            const bool use_tc = tc && tc->ls_tc && cp_gemm_tc_enabled() && n >= 256 && g0 >= 512;
-            if (use_tc || cpgemm::num_tiles(n, g0, cpgemm::TILES_ALL) >= 2 * device_sms())
-                rc = dgemm_big_nc(Wt + g0, ldw, L + (int64_t)g0 * ld, ld, F, ldf, n, g0, gs, -1.0, 1.0, stream,
-                                  use_tc ? tc : nullptr);
-            else
-                rc = dgemm_small<true>(Wt + g0, ldw, L + (int64_t)g0 * ld, ld, F, ldf, n, g0, gs, -1.0, 1.0,
-                                       cpsmall::TILES_ALL, stream);
+            const bool use_tc = tc && h->ls_tc && n >= 256 && g0 >= 512;
+            const int tile = use_tc || num_tiles(n, g0, TILES_ALL, BM) >= 2 * h->num_sms ? 128 : 64;
+            rc = dgemm<true>(h, use_tc, tile, TILES_ALL, 0, Wt + g0, ldw, L + (int64_t)g0 * ld, ld, F, ldf, n, g0, gs, -1.0,
+                             1.0, stream);
             if (rc) return rc;
         }
     }
@@ -839,7 +755,7 @@ extern "C" int cp_ls_solve(cp_handle_t h, const double *G, const double *Bxy, co
     CP_CHECK_LAUNCH();
     rc = chol_factor(h, M, L, ld, Ksel, n, Linv, Tm, diag0, info_out, ratio, stream);
     if (rc) return rc;
-    rc = chol_backward(L, ld, Ksel, Linv, L + (int64_t)Ksel * ld, ld, Wt, ld, n, stream, h);
+    rc = chol_backward(h, true, L, ld, Ksel, Linv, L + (int64_t)Ksel * ld, ld, Wt, ld, n, stream);
     if (rc) return rc;
     ls_output<<<n, 256, 0, stream>>>(Wt, ld, sx, sy, sel_cols, Ksel, invN, W_out, b_out, 0);
     CP_CHECK_LAUNCH();
@@ -924,9 +840,9 @@ extern "C" int cp_ls_resolve(cp_handle_t h, const double *Bxy, const double *sx,
     const double invN = 1.0 / (double)h->fac_N;
     rhs_assemble<<<dim3(cp_cdiv(Ksel, 256), n), 256, 0, stream>>>(Bxy, sx, sy, invN, n, sel_cols, Ksel, Zt, ld);
     CP_CHECK_LAUNCH();
-    rc = chol_forward(L, ld, Ksel, Linv, Zt, F, ld, n, stream, h);
+    rc = chol_forward(h, L, ld, Ksel, Linv, Zt, F, ld, n, stream);
     if (rc) return rc;
-    rc = chol_backward(L, ld, Ksel, Linv, F, ld, Wt, ld, n, stream, h);
+    rc = chol_backward(h, true, L, ld, Ksel, Linv, F, ld, Wt, ld, n, stream);
     if (rc) return rc;
     ls_output<<<n, 256, 0, stream>>>(Wt, ld, sx, sy, sel_cols, Ksel, invN, W_out, b_out, accumulate);
     CP_CHECK_LAUNCH();
@@ -1024,7 +940,7 @@ extern "C" int cp_ls_residual(cp_handle_t h, const float *X, int64_t N, int K, i
     const int64_t ldw = ld_for(K);
     // X Wf' in fp64 (exact products of fp32 data with the fp64 weights): 128 x 128 tiles, reduction split so that the
     // tile count fills whole waves of the SMs (5000 x 512 is 160 tiles on 132 SMs: two waves for 1.2 waves of work)
-    const int tiles = num_tiles((int)N, n, TILES_ALL);
+    const int tiles = num_tiles((int)N, n, TILES_ALL, BM);
     int nsplit = 1;
     double best = 1e30;
     for (int ns = 1; ns <= 6; ++ns) {
@@ -1193,7 +1109,7 @@ extern "C" int cp_ls_solve_dual(cp_handle_t h, const float *X, int64_t N, int K,
     center_sel<<<dim3(cp_cdiv(Ksel, 256), Ni), 256, 0, stream>>>(X, ldx, sel_cols, Ksel, xmean, Xc, ldc);
     CP_CHECK_LAUNCH();
     // H = Xc Xc' (lower tiles) + 1/N
-    rc = dgemm_big(Xc, ldc, Xc, ldc, M, ldm, Ni, Ni, Ksel, 1.0, 0.0, TILES_LOWER, stream);
+    rc = dgemm<false>(h, false, 128, TILES_LOWER, 0, Xc, ldc, Xc, ldc, M, ldm, Ni, Ni, Ksel, 1.0, 0.0, stream);
     if (rc) return rc;
     add_const_lower<<<dim3(cp_cdiv(Ni, 256), Ni), 256, 0, stream>>>(M, ldm, Ni, 1.0 / (double)N, diag0);
     CP_CHECK_LAUNCH();
@@ -1204,19 +1120,11 @@ extern "C" int cp_ls_solve_dual(cp_handle_t h, const float *X, int64_t N, int K,
     CP_CHECK_LAUNCH();
     rc = chol_factor(h, M, L, ldm, Ni, n, Linv, Tm, diag0, info_out, ratio, stream);
     if (rc) return rc;
-    rc = chol_backward(L, ldm, Ni, Linv, L + (int64_t)Ni * ldm, ldm, At, ldm, n, stream);
+    rc = chol_backward(h, false, L, ldm, Ni, Linv, L + (int64_t)Ni * ldm, ldm, At, ldm, n, stream);
     if (rc) return rc;
     // Wt = At * Xc   (C[t, i] = sum_r At[t, r] * Xc[r, i])
-    {
-        Args g{};
-        g.A = At; g.lda = ldm; g.B = Xc; g.ldb = ldc; g.C = Wt; g.ldc = ldc;
-        g.M = n; g.Nn = Ksel; g.R = Ni;
-        g.nsplit = 1; g.r_per_split = Ni;
-        g.alpha = 1.0; g.beta = 0.0; g.tile_mode = TILES_ALL;
-        g.a_vec = al16(At) && (ldm % 2 == 0);
-        g.b_vec = al16(Xc) && (ldc % 2 == 0);
-        CP_GEMM_LAUNCH((launch<double, double, false, true>(g, stream)));
-    }
+    rc = dgemm<true>(h, false, 128, TILES_ALL, 0, At, ldm, Xc, ldc, Wt, ldc, n, Ksel, Ni, 1.0, 0.0, stream);
+    if (rc) return rc;
     dual_output<<<n, 256, 0, stream>>>(Wt, ldc, xmean, ymean, Ksel, W_out, b_out);
     CP_CHECK_LAUNCH();
     if (stat_out) CP_CUDA(cudaMemcpyAsync(stat_out, ratio, sizeof(double), cudaMemcpyDeviceToDevice, stream));

@@ -51,7 +51,7 @@ enum { CP_F32 = 0, CP_F64 = 1 };
 
 /* arithmetic of cp_gram */
 enum {
-    CP_GRAM_FP64 = 0,  /* fp32 inputs widened to fp64, DFMA accumulate (exact products) */
+    CP_GRAM_FP64 = 0,  /* fp32 inputs widened to fp64, DMMA accumulate (exact products) */
     CP_GRAM_3XTF32 = 1 /* tensor cores (wgmma), three products of a 22-bit hi/lo operand split, fp32 register
                           accumulation per 64-row run, fp64 reduction over the runs.  The split is into two fp16
                           halves of the shifted and power-of-two scaled data (the same split precision as tf32 at

@@ -1,4 +1,7 @@
 """fp64 GEMM kernels of libcpb200 (gemm_f64.cuh through cp_gemm_f64) against cuBLAS on the shapes the solver uses.
+cp_gemm_f64 runs the cp.async kernel unless the product has fewer 128 x 128 tiles than twice the SMs and a reduction of
+at least 128: those (the substitution, panel-solve and residual shapes) split the reduction over the register-staged
+kernel.  The solver itself calls the cp.async kernel directly, without a split.
     python profiles/gemm_bench.py
 """
 import os
