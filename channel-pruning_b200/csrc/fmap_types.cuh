@@ -1,0 +1,17 @@
+// Element types of the feature maps the gathers read (CP_F32, CP_BF16, CP_F16).  The gathered matrices X and Y are
+// fp32 whatever the map holds: cp_widen converts exactly (every bf16 and fp16 value, fp16 subnormals included, is an
+// fp32 value), so a 16-bit map gathers to the bits the fp32 map of the same values gives.
+#pragma once
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+
+#include "../../include/cpb200.h"
+
+__device__ __forceinline__ float cp_widen(float v) { return v; }
+__device__ __forceinline__ float cp_widen(__nv_bfloat16 v) { return __bfloat162float(v); }
+__device__ __forceinline__ float cp_widen(__half v) { return __half2float(v); }
+
+// bytes per map element; 0 for a type the gathers do not read (CP_F64, unknown codes)
+static inline int cp_fmap_esize(int fmap_dtype) {
+    return fmap_dtype == CP_F32 ? 4 : (fmap_dtype == CP_BF16 || fmap_dtype == CP_F16) ? 2 : 0;
+}

@@ -13,15 +13,19 @@
 // NHWC path: a window row is k*c contiguous floats; the CTA stages the k*k x c tile
 // in shared memory with coalesced loads (channel fastest) and writes it back
 // transposed to (c, k*k) column order, again coalesced.
+// Element type of the map: fp32, bf16 or fp16 (template parameter T, fmap_types.cuh).  X and Y are fp32 in every
+// case; the ReLU is applied to the widened value with the fp32 kernel's expression, so -0, inf and NaN come out as the
+// fp32 kernel gives them for the widened map.
 #include <cstdlib>
 
 #include "common.cuh"
+#include "fmap_types.cuh"
 
 namespace {
 
-template <int KS>
+template <int KS, typename T>
 __global__ void __launch_bounds__(256)
-patch_gather_nchw(const float *__restrict__ fmap, const int32_t *__restrict__ randx,
+patch_gather_nchw(const T *__restrict__ fmap, const int32_t *__restrict__ randx,
                   const int32_t *__restrict__ randy, float *__restrict__ X, int64_t ldx, int64_t rows, int B, int c,
                   int H, int W, int P, int k_rt, int pad, int stride, int relu) {
     const int k = KS > 0 ? KS : k_rt;
@@ -35,7 +39,7 @@ patch_gather_nchw(const float *__restrict__ fmap, const int32_t *__restrict__ ra
         const int batch = (int)(bp / P);
         const int y0 = stride * randx[bp] - pad;  // window origin, rows   (net.py: feat[:,:,x,y], x indexes H)
         const int x0 = stride * randy[bp] - pad;  // window origin, cols
-        const float *src = fmap + ((int64_t)batch * B + img_in_batch) * c * H * W;
+        const T *src = fmap + ((int64_t)batch * B + img_in_batch) * c * H * W;
         float *dst = X + r * ldx;
 #pragma unroll 4
         for (int col = threadIdx.x; col < K; col += blockDim.x) {
@@ -45,7 +49,7 @@ patch_gather_nchw(const float *__restrict__ fmap, const int32_t *__restrict__ ra
             const int px = p - py * k;
             const int yy = y0 + py, xx = x0 + px;
             float v = 0.f;
-            if (yy >= 0 && yy < H && xx >= 0 && xx < W) v = __ldg(src + ((int64_t)a * H + yy) * W + xx);
+            if (yy >= 0 && yy < H && xx >= 0 && xx < W) v = cp_widen(__ldg(src + ((int64_t)a * H + yy) * W + xx));
             if (relu) v = fmaxf(v, 0.f);
             dst[col] = v;
         }
@@ -57,8 +61,9 @@ constexpr int64_t CP_HOST_GATHER_CTAS = 64;  // grid of the in-place (zero-copy)
 // NHWC: tile = k2 spatial taps x CT channels staged through shared memory.
 constexpr int NHWC_CT = 128;  // channels per tile
 
+template <typename T>
 __global__ void __launch_bounds__(256)
-patch_gather_nhwc(const float *__restrict__ fmap, const int32_t *__restrict__ randx,
+patch_gather_nhwc(const T *__restrict__ fmap, const int32_t *__restrict__ randx,
                   const int32_t *__restrict__ randy, float *__restrict__ X, int64_t ldx, int B, int c, int H,
                   int W, int P, int k, int pad, int stride, int relu) {
     extern __shared__ float tile[];  // [k2][NHWC_CT + 1]
@@ -71,14 +76,14 @@ patch_gather_nhwc(const float *__restrict__ fmap, const int32_t *__restrict__ ra
     const int batch = (int)(bp / P);
     const int y0 = stride * randx[bp] - pad;
     const int x0 = stride * randy[bp] - pad;
-    const float *src = fmap + ((int64_t)batch * B + img_in_batch) * H * W * c;
+    const T *src = fmap + ((int64_t)batch * B + img_in_batch) * H * W * c;
     for (int e = threadIdx.x; e < k2 * ct; e += blockDim.x) {
         const int p = e / ct;
         const int a = e - p * ct;
         const int py = p / k, px = p - py * k;
         const int yy = y0 + py, xx = x0 + px;
         float v = 0.f;
-        if (yy >= 0 && yy < H && xx >= 0 && xx < W) v = __ldg(src + ((int64_t)yy * W + xx) * c + a0 + a);
+        if (yy >= 0 && yy < H && xx >= 0 && xx < W) v = cp_widen(__ldg(src + ((int64_t)yy * W + xx) * c + a0 + a));
         if (relu) v = fmaxf(v, 0.f);
         tile[p * (NHWC_CT + 1) + a] = v;
     }
@@ -91,8 +96,9 @@ patch_gather_nhwc(const float *__restrict__ fmap, const int32_t *__restrict__ ra
     }
 }
 
+template <typename T>
 __global__ void __launch_bounds__(256)
-point_gather(const float *__restrict__ fmap, const int32_t *__restrict__ randx,
+point_gather(const T *__restrict__ fmap, const int32_t *__restrict__ randx,
              const int32_t *__restrict__ randy, float *__restrict__ Y, int64_t ldy, int B, int n, int H, int W,
              int P, int nhwc) {
     const int64_t r = blockIdx.x;
@@ -100,24 +106,24 @@ point_gather(const float *__restrict__ fmap, const int32_t *__restrict__ randx,
     const int64_t bp = r / B;
     const int batch = (int)(bp / P);
     const int yy = randx[bp], xx = randy[bp];
-    const float *src = fmap + ((int64_t)batch * B + img_in_batch) * n * H * W;
+    const T *src = fmap + ((int64_t)batch * B + img_in_batch) * n * H * W;
     float *dst = Y + r * ldy;
     if (nhwc) {
-        const float *s = src + ((int64_t)yy * W + xx) * n;
-        for (int j = threadIdx.x; j < n; j += blockDim.x) dst[j] = __ldg(s + j);
+        const T *s = src + ((int64_t)yy * W + xx) * n;
+        for (int j = threadIdx.x; j < n; j += blockDim.x) dst[j] = cp_widen(__ldg(s + j));
     } else {
-        const float *s = src + (int64_t)yy * W + xx;
-        for (int j = threadIdx.x; j < n; j += blockDim.x) dst[j] = __ldg(s + (int64_t)j * H * W);
+        const T *s = src + (int64_t)yy * W + xx;
+        for (int j = threadIdx.x; j < n; j += blockDim.x) dst[j] = cp_widen(__ldg(s + (int64_t)j * H * W));
     }
 }
 
 }  // namespace
 
 // gather_tma.cu
-bool cp_gather_tma_eligible(const float *fmap, int c, int k, float *X_out, int64_t ldx);
-int cp_patch_gather_tma(cp_handle_t h, const float *fmap, int nbatch, int B, int c, int H, int W, const int32_t *randx,
-                        const int32_t *randy, int P, int k, int pad, int stride, int relu, float *X_out, int64_t ldx,
-                        cudaStream_t stream);
+bool cp_gather_tma_eligible(const void *fmap, int esize, int c, int k, float *X_out, int64_t ldx);
+int cp_patch_gather_tma(cp_handle_t h, const void *fmap, int fmap_dtype, int nbatch, int B, int c, int H, int W,
+                        const int32_t *randx, const int32_t *randy, int P, int k, int pad, int stride, int relu,
+                        float *X_out, int64_t ldx, cudaStream_t stream);
 static bool tma_enabled() {  // CPB200_GATHER_TMA=0 keeps the SIMT kernel (A/B measurements)
     static const bool on = [] {
         const char *e = getenv("CPB200_GATHER_TMA");
@@ -126,9 +132,32 @@ static bool tma_enabled() {  // CPB200_GATHER_TMA=0 keeps the SIMT kernel (A/B m
     return on;
 }
 
-extern "C" int cp_patch_gather(cp_handle_t h, const float *fmap, int nbatch, int B, int c, int H, int W,
-                               int layout, const int32_t *randx, const int32_t *randy, int P, int k, int pad,
-                               int stride, int relu, float *X_out, int64_t ldx, cp_stream_t stream_) {
+template <typename T>
+static void launch_patch_gather_simt(const T *fmap, int layout, bool host_src, int64_t host_ctas, int64_t rows,
+                                     int B, int c, int H, int W, const int32_t *randx, const int32_t *randy, int P,
+                                     int k, int pad, int stride, int relu, float *X_out, int64_t ldx,
+                                     cudaStream_t stream) {
+    if (layout == CP_LAYOUT_NCHW) {
+        const int64_t ncta = host_src ? (rows < host_ctas ? rows : host_ctas) : rows;
+        dim3 grid((unsigned)ncta);
+        if (k == 3)
+            patch_gather_nchw<3><<<grid, 256, 0, stream>>>(fmap, randx, randy, X_out, ldx, rows, B, c, H, W, P, k, pad, stride, relu);
+        else if (k == 1)
+            patch_gather_nchw<1><<<grid, 256, 0, stream>>>(fmap, randx, randy, X_out, ldx, rows, B, c, H, W, P, k, pad, stride, relu);
+        else
+            patch_gather_nchw<0><<<grid, 256, 0, stream>>>(fmap, randx, randy, X_out, ldx, rows, B, c, H, W, P, k, pad, stride, relu);
+    } else {
+        const size_t smem = (size_t)k * k * (NHWC_CT + 1) * sizeof(float);
+        dim3 grid((unsigned)rows, (unsigned)cp_cdiv(c, NHWC_CT));
+        patch_gather_nhwc<<<grid, 256, smem, stream>>>(fmap, randx, randy, X_out, ldx, B, c, H, W, P, k, pad, stride, relu);
+    }
+}
+
+extern "C" int cp_patch_gather_typed(cp_handle_t h, const void *fmap, int fmap_dtype, int nbatch, int B, int c, int H,
+                                     int W, int layout, const int32_t *randx, const int32_t *randy, int P, int k,
+                                     int pad, int stride, int relu, float *X_out, int64_t ldx, cp_stream_t stream_) {
+    const int esize = cp_fmap_esize(fmap_dtype);
+    CP_REQUIRE(esize, "cp_patch_gather: feature-map dtype %d is not CP_F32, CP_BF16 or CP_F16", fmap_dtype);
     CP_REQUIRE(h && fmap && randx && randy && X_out, "cp_patch_gather: NULL argument");
     CP_REQUIRE(nbatch >= 0 && B > 0 && c > 0 && H > 0 && W > 0 && P > 0, "cp_patch_gather: bad shape");
     CP_REQUIRE(k >= 1 && (k & 1) == 1, "cp_patch_gather: kernel_size must be odd (reference net.py:604-605), got %d", k);
@@ -139,40 +168,52 @@ extern "C" int cp_patch_gather(cp_handle_t h, const float *fmap, int nbatch, int
     const int64_t rows = (int64_t)nbatch * P * B;
     if (rows == 0) return CP_OK;
     CP_REQUIRE(rows < (1ll << 31), "cp_patch_gather: too many rows");
+    bool host_src = false;
+    int64_t host_ctas = CP_HOST_GATHER_CTAS;
     if (layout == CP_LAYOUT_NCHW) {
         // map in (pinned, UVA-mapped) host memory?  then the kernel is a PCIe reader: keep its footprint small
         cudaPointerAttributes pa;
-        const bool host_src = cudaPointerGetAttributes(&pa, fmap) == cudaSuccess && pa.type == cudaMemoryTypeHost;
+        host_src = cudaPointerGetAttributes(&pa, fmap) == cudaSuccess && pa.type == cudaMemoryTypeHost;
         (void)cudaGetLastError();
-        static const int64_t host_ctas = [] {
+        static const int64_t env_host_ctas = [] {
             const char *e = getenv("CPB200_HOST_GATHER_CTAS");  // tuning knob (profiles/e2e_breakdown.py)
             const long v = e ? atol(e) : 0;
             return (int64_t)(v > 0 ? v : CP_HOST_GATHER_CTAS);
         }();
-        const int64_t ncta = host_src ? (rows < host_ctas ? rows : host_ctas) : rows;
-        dim3 grid((unsigned)ncta);
-        if (k == 3)
-            patch_gather_nchw<3><<<grid, 256, 0, stream>>>(fmap, randx, randy, X_out, ldx, rows, B, c, H, W, P, k, pad, stride, relu);
-        else if (k == 1)
-            patch_gather_nchw<1><<<grid, 256, 0, stream>>>(fmap, randx, randy, X_out, ldx, rows, B, c, H, W, P, k, pad, stride, relu);
-        else
-            patch_gather_nchw<0><<<grid, 256, 0, stream>>>(fmap, randx, randy, X_out, ldx, rows, B, c, H, W, P, k, pad, stride, relu);
-    } else if (tma_enabled() && cp_gather_tma_eligible(fmap, c, k, X_out, ldx)) {
+        host_ctas = env_host_ctas;
+    } else if (tma_enabled() && cp_gather_tma_eligible(fmap, esize, c, k, X_out, ldx)) {
         // NHWC map in HBM: whole windows by TMA, rows out by bulk store (gather_tma.cu)
-        return cp_patch_gather_tma(h, fmap, nbatch, B, c, H, W, randx, randy, P, k, pad, stride, relu, X_out, ldx, stream);
+        return cp_patch_gather_tma(h, fmap, fmap_dtype, nbatch, B, c, H, W, randx, randy, P, k, pad, stride, relu,
+                                   X_out, ldx, stream);
     } else {
         const size_t smem = (size_t)k * k * (NHWC_CT + 1) * sizeof(float);
         CP_REQUIRE(smem <= 48 * 1024, "cp_patch_gather: kernel_size %d too large for the NHWC tile", k);
-        dim3 grid((unsigned)rows, (unsigned)cp_cdiv(c, NHWC_CT));
-        patch_gather_nhwc<<<grid, 256, smem, stream>>>(fmap, randx, randy, X_out, ldx, B, c, H, W, P, k, pad, stride, relu);
     }
+    if (fmap_dtype == CP_F32)
+        launch_patch_gather_simt((const float *)fmap, layout, host_src, host_ctas, rows, B, c, H, W, randx, randy, P,
+                                 k, pad, stride, relu, X_out, ldx, stream);
+    else if (fmap_dtype == CP_BF16)
+        launch_patch_gather_simt((const __nv_bfloat16 *)fmap, layout, host_src, host_ctas, rows, B, c, H, W, randx,
+                                 randy, P, k, pad, stride, relu, X_out, ldx, stream);
+    else
+        launch_patch_gather_simt((const __half *)fmap, layout, host_src, host_ctas, rows, B, c, H, W, randx, randy, P,
+                                 k, pad, stride, relu, X_out, ldx, stream);
     CP_CHECK_LAUNCH();
     return CP_OK;
 }
 
-extern "C" int cp_point_gather(cp_handle_t h, const float *fmap, int nbatch, int B, int n, int H, int W,
-                               int layout, const int32_t *randx, const int32_t *randy, int P, float *Y_out,
-                               int64_t ldy, cp_stream_t stream_) {
+extern "C" int cp_patch_gather(cp_handle_t h, const float *fmap, int nbatch, int B, int c, int H, int W,
+                               int layout, const int32_t *randx, const int32_t *randy, int P, int k, int pad,
+                               int stride, int relu, float *X_out, int64_t ldx, cp_stream_t stream_) {
+    return cp_patch_gather_typed(h, fmap, CP_F32, nbatch, B, c, H, W, layout, randx, randy, P, k, pad, stride, relu,
+                                 X_out, ldx, stream_);
+}
+
+extern "C" int cp_point_gather_typed(cp_handle_t h, const void *fmap, int fmap_dtype, int nbatch, int B, int n, int H,
+                                     int W, int layout, const int32_t *randx, const int32_t *randy, int P,
+                                     float *Y_out, int64_t ldy, cp_stream_t stream_) {
+    CP_REQUIRE(cp_fmap_esize(fmap_dtype), "cp_point_gather: feature-map dtype %d is not CP_F32, CP_BF16 or CP_F16",
+               fmap_dtype);
     CP_REQUIRE(h && fmap && randx && randy && Y_out, "cp_point_gather: NULL argument");
     CP_REQUIRE(nbatch >= 0 && B > 0 && n > 0 && H > 0 && W > 0 && P > 0, "cp_point_gather: bad shape");
     CP_REQUIRE(ldy >= n, "cp_point_gather: ldy < n");
@@ -180,8 +221,22 @@ extern "C" int cp_point_gather(cp_handle_t h, const float *fmap, int nbatch, int
     const int64_t rows = (int64_t)nbatch * P * B;
     if (rows == 0) return CP_OK;
     CP_REQUIRE(rows < (1ll << 31), "cp_point_gather: too many rows");
-    point_gather<<<(unsigned)rows, 256, 0, (cudaStream_t)stream_>>>(fmap, randx, randy, Y_out, ldy, B, n, H, W, P,
-                                                                   layout == CP_LAYOUT_NHWC);
+    const cudaStream_t stream = (cudaStream_t)stream_;
+    const int nhwc = layout == CP_LAYOUT_NHWC;
+    if (fmap_dtype == CP_F32)
+        point_gather<<<(unsigned)rows, 256, 0, stream>>>((const float *)fmap, randx, randy, Y_out, ldy, B, n, H, W, P, nhwc);
+    else if (fmap_dtype == CP_BF16)
+        point_gather<<<(unsigned)rows, 256, 0, stream>>>((const __nv_bfloat16 *)fmap, randx, randy, Y_out, ldy, B, n, H,
+                                                         W, P, nhwc);
+    else
+        point_gather<<<(unsigned)rows, 256, 0, stream>>>((const __half *)fmap, randx, randy, Y_out, ldy, B, n, H, W, P,
+                                                         nhwc);
     CP_CHECK_LAUNCH();
     return CP_OK;
+}
+
+extern "C" int cp_point_gather(cp_handle_t h, const float *fmap, int nbatch, int B, int n, int H, int W,
+                               int layout, const int32_t *randx, const int32_t *randy, int P, float *Y_out,
+                               int64_t ldy, cp_stream_t stream_) {
+    return cp_point_gather_typed(h, fmap, CP_F32, nbatch, B, n, H, W, layout, randx, randy, P, Y_out, ldy, stream_);
 }

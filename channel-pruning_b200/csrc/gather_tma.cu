@@ -14,11 +14,15 @@
 //     one consumer      bulk store of the row, two rows in flight
 // Bytes: the window is read once and the row written once -- 8 N K bytes, the algorithmic figure of SURVEY.md 8(d).
 // Bound: HBM.
+// bf16 / fp16 maps (template parameter T): the tensor map has the 16-bit data type, the window stage holds 16-bit
+// elements (half the bytes), and the consumers widen exactly while transposing; the row stays fp32.  6 N K bytes.
+// The 16-byte rules of TMA (global strides, box rows) then need c % 8 == 0.
 #include <cuda.h>
 
 #include <cstdlib>
 
 #include "common.cuh"
+#include "fmap_types.cuh"
 
 namespace {
 
@@ -31,7 +35,7 @@ struct GtParams {
     float *X;
     int64_t ldx, rows;
     int B, P, c, k, pad, stride, relu, cbox, nbox, nstage;
-    int box_f, stage_f, out_f;  // strides in floats, each a multiple of 32 (TMA destinations are 128-byte aligned)
+    int box_f, stage_f, out_f;  // strides in map elements (box, stage) and floats (out); 128-byte multiples each
 };
 
 __device__ __forceinline__ uint32_t g_smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -68,16 +72,16 @@ __device__ __forceinline__ void g_bulk_store(void *gdst, uint32_t ssrc, uint32_t
 }
 __device__ __forceinline__ void g_cons_barrier() { asm volatile("bar.sync 1, %0;" ::"n"(GT_CONS) : "memory"); }
 
-template <int K2>  // k*k known at compile time (1, 9, 25) or 0
+template <typename T, int K2>  // map element type; k*k known at compile time (1, 9, 25) or 0
 __global__ void __launch_bounds__(GT_THREADS)
 patch_gather_nhwc_tma(const __grid_constant__ CUtensorMap map, const GtParams P) {
     extern __shared__ __align__(128) unsigned char gsm_raw[];
     const int k2 = K2 > 0 ? K2 : P.k * P.k, K = P.c * k2;
-    const uint32_t stage_bytes = (uint32_t)K * 4u;
-    // layout: [nstage][K] input windows ([box][tap][c_box]), [GT_OUT][K] output rows, mbarriers
+    const uint32_t stage_bytes = (uint32_t)K * (uint32_t)sizeof(T), row_bytes = (uint32_t)K * 4u;
+    // layout: [nstage][K] input windows ([box][tap][c_box], type T), [GT_OUT][K] fp32 output rows, mbarriers
     unsigned char *base = (unsigned char *)(((uintptr_t)gsm_raw + 127) & ~(uintptr_t)127);
-    float *in = reinterpret_cast<float *>(base);
-    float *out = in + (size_t)P.nstage * P.stage_f;
+    T *in = reinterpret_cast<T *>(base);
+    float *out = reinterpret_cast<float *>(in + (size_t)P.nstage * P.stage_f);
     uint64_t *bars = reinterpret_cast<uint64_t *>(out + (size_t)GT_OUT * P.out_f);  // full[nstage], empty[nstage]
     const int tid = threadIdx.x;
     const uint32_t bar0 = g_smem_u32(bars);
@@ -120,7 +124,8 @@ patch_gather_nhwc_tma(const __grid_constant__ CUtensorMap map, const GtParams P)
                     g_mbar_expect_tx(full(s), stage_bytes);
                     const uint32_t dst = g_smem_u32(in + (size_t)s * P.stage_f);
                     for (int b = 0; b < P.nbox; ++b)
-                        g_tma_load_4d(dst + (uint32_t)b * (uint32_t)P.box_f * 4u, &map, full(s), b * P.cbox, xs, ys, is);
+                        g_tma_load_4d(dst + (uint32_t)b * (uint32_t)P.box_f * (uint32_t)sizeof(T), &map, full(s),
+                                      b * P.cbox, xs, ys, is);
                 }
                 __syncwarp();
             }
@@ -135,21 +140,21 @@ patch_gather_nhwc_tma(const __grid_constant__ CUtensorMap map, const GtParams P)
         g_mbar_wait(full(s), ph);
         if (tid == 0 && it >= GT_OUT) asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(GT_OUT - 1) : "memory");
         g_cons_barrier();  // out[o] is no longer being read by the store of row it - GT_OUT
-        const float *src = in + (size_t)s * P.stage_f;
+        const T *src = in + (size_t)s * P.stage_f;
         float *dst = out + (size_t)o * P.out_f;
         for (int a = tid; a < P.c; a += GT_CONS) {
             const int b = a / P.cbox, al = a - b * P.cbox;
-            const float *sp = src + (size_t)b * P.box_f + al;
+            const T *sp = src + (size_t)b * P.box_f + al;
             float *dp = dst + (size_t)a * k2;
             if (K2 > 0) {
                 float v[K2 > 0 ? K2 : 1];
 #pragma unroll
-                for (int p = 0; p < K2; ++p) v[p] = sp[p * P.cbox];
+                for (int p = 0; p < K2; ++p) v[p] = cp_widen(sp[p * P.cbox]);
 #pragma unroll
                 for (int p = 0; p < K2; ++p) dp[p] = P.relu ? fmaxf(v[p], 0.f) : v[p];
             } else {
                 for (int p = 0; p < k2; ++p) {
-                    float v = sp[(size_t)p * P.cbox];
+                    float v = cp_widen(sp[(size_t)p * P.cbox]);
                     if (P.relu) v = fmaxf(v, 0.f);
                     dp[p] = v;
                 }
@@ -159,7 +164,7 @@ patch_gather_nhwc_tma(const __grid_constant__ CUtensorMap map, const GtParams P)
         g_cons_barrier();
         if (tid == 0) {
             g_mbar_arrive(empty(s));  // every consumer has finished reading in[s]
-            g_bulk_store(P.X + r * P.ldx, g_smem_u32(dst), stage_bytes);
+            g_bulk_store(P.X + r * P.ldx, g_smem_u32(dst), row_bytes);
             asm volatile("cp.async.bulk.commit_group;" ::: "memory");
         }
     }
@@ -174,69 +179,12 @@ typedef CUresult (*encode_fn_t)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, 
 
 }  // namespace
 
-// true when the TMA path applies (device memory, 16-byte rules); the caller falls back to the SIMT kernel otherwise
-bool cp_gather_tma_eligible(const float *fmap, int c, int k, float *X_out, int64_t ldx) {
-    if (c % 4 || c < 16 || k > 16) return false;
-    if (((uintptr_t)fmap & 15) || ((uintptr_t)X_out & 15) || (ldx % 4)) return false;
-    cudaPointerAttributes pa;
-    if (cudaPointerGetAttributes(&pa, fmap) != cudaSuccess || pa.type != cudaMemoryTypeDevice) {
-        (void)cudaGetLastError();
-        return false;
-    }
-    int cbox = 0;
-    for (int d = 256; d >= 16; d -= 4)
-        if (c % d == 0) { cbox = d; break; }
-    if (!cbox) return false;
-    const size_t row = gt_round128((size_t)cbox * k * k * 4) * (c / cbox);
-    return (2 + GT_OUT) * row + 1024 <= 200 * 1024;  // at least two input stages in one CTA
-}
-
-int cp_patch_gather_tma(cp_handle_t h, const float *fmap, int nbatch, int B, int c, int H, int W, const int32_t *randx,
-                        const int32_t *randy, int P, int k, int pad, int stride, int relu, float *X_out, int64_t ldx,
-                        cudaStream_t stream) {
-    if (!h->tmap_encode) {
-        void *fn = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        CP_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
-        if (!fn || qres != cudaDriverEntryPointSuccess) CP_FAIL(CP_ERR_CUDA, "cuTensorMapEncodeTiled not available");
-        h->tmap_encode = fn;
-    }
-    int cbox = 0;
-    for (int d = 256; d >= 16; d -= 4)
-        if (c % d == 0) { cbox = d; break; }
-    const int64_t nimg = (int64_t)nbatch * B;
-    CUtensorMap map;
-    const cuuint64_t dims[4] = {(cuuint64_t)c, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)nimg};
-    const cuuint64_t strides[3] = {(cuuint64_t)c * 4, (cuuint64_t)W * c * 4, (cuuint64_t)H * W * c * 4};
-    const cuuint32_t box[4] = {(cuuint32_t)cbox, (cuuint32_t)k, (cuuint32_t)k, 1};
-    const cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult cr = ((encode_fn_t)h->tmap_encode)(&map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void *)fmap, dims, strides, box, estr,
-                                                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-                                                CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) CP_FAIL(CP_ERR_CUDA, "cuTensorMapEncodeTiled (4-D feature map) failed (%d)", (int)cr);
-    GtParams Pm{};
-    Pm.randx = randx; Pm.randy = randy; Pm.X = X_out; Pm.ldx = ldx;
-    Pm.rows = (int64_t)nbatch * P * B;
-    Pm.B = B; Pm.P = P; Pm.c = c; Pm.k = k; Pm.pad = pad; Pm.stride = stride; Pm.relu = relu;
-    Pm.cbox = cbox; Pm.nbox = c / cbox;
-    const size_t box_b = gt_round128((size_t)cbox * k * k * 4), row = box_b * Pm.nbox;
-    const size_t out_b = gt_round128((size_t)c * k * k * 4);
-    // CTAs per SM: as many as fit with >= 2 input stages each (up to 4), then the stages fill what is left
-    const size_t budget = 216 * 1024;
-    int per_sm = (int)(budget / (2 * row + GT_OUT * out_b + 1024));
-    per_sm = per_sm < 1 ? 1 : (per_sm > 4 ? 4 : per_sm);
-    static const int env_per_sm = [] { const char *e = getenv("CPB200_GATHER_CTAS_PER_SM"); return e ? atoi(e) : 0; }();
-    static const int env_stages = [] { const char *e = getenv("CPB200_GATHER_STAGES"); return e ? atoi(e) : 0; }();
-    if (env_per_sm > 0 && env_per_sm < per_sm) per_sm = env_per_sm;  // tuning knobs
-    int nstage = (int)((budget / per_sm - 1024 - GT_OUT * out_b) / row);
-    if (nstage > 6) nstage = 6;
-    if (env_stages >= 2 && env_stages < nstage) nstage = env_stages;
-    Pm.nstage = nstage;
-    Pm.box_f = (int)(box_b / 4); Pm.stage_f = (int)(row / 4); Pm.out_f = (int)(out_b / 4);
-    const size_t smem = (size_t)nstage * row + GT_OUT * out_b + 2 * nstage * 8 + 256;
-    auto kern = k == 3 ? patch_gather_nhwc_tma<9> : k == 1 ? patch_gather_nhwc_tma<1> : k == 5 ? patch_gather_nhwc_tma<25>
-                                                                                              : patch_gather_nhwc_tma<0>;
-    static cp_per_device_flag configured[4];
+template <typename T>
+static int gt_launch(cp_handle_t h, const CUtensorMap &map, const GtParams &Pm, int k, size_t smem, int per_sm,
+                     cudaStream_t stream) {
+    auto kern = k == 3 ? patch_gather_nhwc_tma<T, 9> : k == 1 ? patch_gather_nhwc_tma<T, 1>
+              : k == 5 ? patch_gather_nhwc_tma<T, 25> : patch_gather_nhwc_tma<T, 0>;
+    static cp_per_device_flag configured[4];  // one set per element type (one per instantiation of gt_launch)
     const int which = k == 3 ? 0 : k == 1 ? 1 : k == 5 ? 2 : 3;
     if (bool *done = configured[which].slot(); !*done) {
         CP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
@@ -247,4 +195,80 @@ int cp_patch_gather_tma(cp_handle_t h, const float *fmap, int nbatch, int B, int
     kern<<<(unsigned)grid, GT_THREADS, smem, stream>>>(map, Pm);
     CP_CHECK_LAUNCH();
     return CP_OK;
+}
+
+// Channels per TMA box: the largest divisor of c in [16, 256] whose box row is a multiple of 16 bytes (TMA), 0 if none
+static int gt_cbox(int c, int esize) {
+    for (int d = 256; d >= 16; d -= 16 / esize)
+        if (c % d == 0) return d;
+    return 0;
+}
+
+// true when the TMA path applies (device memory, 16-byte rules); the caller falls back to the SIMT kernel otherwise
+bool cp_gather_tma_eligible(const void *fmap, int esize, int c, int k, float *X_out, int64_t ldx) {
+    if (c % (16 / esize) || c < 16 || k > 16) return false;
+    if (((uintptr_t)fmap & 15) || ((uintptr_t)X_out & 15) || (ldx % 4)) return false;
+    cudaPointerAttributes pa;
+    if (cudaPointerGetAttributes(&pa, fmap) != cudaSuccess || pa.type != cudaMemoryTypeDevice) {
+        (void)cudaGetLastError();
+        return false;
+    }
+    const int cbox = gt_cbox(c, esize);
+    if (!cbox) return false;
+    // a window stage and an output row; for fp32 the stage is never smaller than the row
+    const size_t row = gt_round128((size_t)cbox * k * k * esize) * (c / cbox);
+    const size_t out_b = gt_round128((size_t)c * k * k * 4);
+    return 2 * row + GT_OUT * (row > out_b ? row : out_b) + 1024 <= 200 * 1024;  // at least two input stages in one CTA
+}
+
+int cp_patch_gather_tma(cp_handle_t h, const void *fmap, int fmap_dtype, int nbatch, int B, int c, int H, int W,
+                        const int32_t *randx, const int32_t *randy, int P, int k, int pad, int stride, int relu,
+                        float *X_out, int64_t ldx, cudaStream_t stream) {
+    if (!h->tmap_encode) {
+        void *fn = nullptr;
+        cudaDriverEntryPointQueryResult qres;
+        CP_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
+        if (!fn || qres != cudaDriverEntryPointSuccess) CP_FAIL(CP_ERR_CUDA, "cuTensorMapEncodeTiled not available");
+        h->tmap_encode = fn;
+    }
+    const int esize = cp_fmap_esize(fmap_dtype);
+    const int cbox = gt_cbox(c, esize);
+    const int64_t nimg = (int64_t)nbatch * B;
+    CUtensorMap map;
+    const cuuint64_t dims[4] = {(cuuint64_t)c, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)nimg};
+    const cuuint64_t strides[3] = {(cuuint64_t)c * esize, (cuuint64_t)W * c * esize, (cuuint64_t)H * W * c * esize};
+    const cuuint32_t box[4] = {(cuuint32_t)cbox, (cuuint32_t)k, (cuuint32_t)k, 1};
+    const cuuint32_t estr[4] = {1, 1, 1, 1};
+    const CUtensorMapDataType dt = fmap_dtype == CP_BF16  ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                   : fmap_dtype == CP_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
+                                                          : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+    CUresult cr = ((encode_fn_t)h->tmap_encode)(&map, dt, 4, (void *)fmap, dims, strides, box, estr,
+                                                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+                                                CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (cr != CUDA_SUCCESS) CP_FAIL(CP_ERR_CUDA, "cuTensorMapEncodeTiled (4-D feature map) failed (%d)", (int)cr);
+    GtParams Pm{};
+    Pm.randx = randx; Pm.randy = randy; Pm.X = X_out; Pm.ldx = ldx;
+    Pm.rows = (int64_t)nbatch * P * B;
+    Pm.B = B; Pm.P = P; Pm.c = c; Pm.k = k; Pm.pad = pad; Pm.stride = stride; Pm.relu = relu;
+    Pm.cbox = cbox; Pm.nbox = c / cbox;
+    const size_t box_b = gt_round128((size_t)cbox * k * k * esize), row = box_b * Pm.nbox;
+    const size_t out_b = gt_round128((size_t)c * k * k * 4);
+    // CTAs per SM: as many as fit with >= 2 input stages each (up to 4), then the stages fill what is left.
+    // conv4_x (c = 512, k = 3): fp32 stage 18 KB, row 18 KB -> 2 CTAs x 3 stages; 16-bit stage 9 KB, row 18 KB ->
+    // 3 CTAs x 3 stages (the fp32 output rows then take most of the budget)
+    const size_t budget = 216 * 1024;
+    int per_sm = (int)(budget / (2 * row + GT_OUT * out_b + 1024));
+    per_sm = per_sm < 1 ? 1 : (per_sm > 4 ? 4 : per_sm);
+    static const int env_per_sm = [] { const char *e = getenv("CPB200_GATHER_CTAS_PER_SM"); return e ? atoi(e) : 0; }();
+    static const int env_stages = [] { const char *e = getenv("CPB200_GATHER_STAGES"); return e ? atoi(e) : 0; }();
+    if (env_per_sm > 0 && env_per_sm < per_sm) per_sm = env_per_sm;  // tuning knobs
+    int nstage = (int)((budget / per_sm - 1024 - GT_OUT * out_b) / row);
+    if (nstage > 6) nstage = 6;
+    if (env_stages >= 2 && env_stages < nstage) nstage = env_stages;
+    Pm.nstage = nstage;
+    Pm.box_f = (int)(box_b / esize); Pm.stage_f = (int)(row / esize); Pm.out_f = (int)(out_b / 4);
+    const size_t smem = (size_t)nstage * row + GT_OUT * out_b + 2 * nstage * 8 + 256;
+    if (fmap_dtype == CP_BF16) return gt_launch<__nv_bfloat16>(h, map, Pm, k, smem, per_sm, stream);
+    if (fmap_dtype == CP_F16) return gt_launch<__half>(h, map, Pm, k, smem, per_sm, stream);
+    return gt_launch<float>(h, map, Pm, k, smem, per_sm, stream);
 }

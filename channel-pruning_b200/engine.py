@@ -43,6 +43,16 @@ DEFER_FULL_GRAM = os.environ.get("CPB200_DEFER_GRAM", "1") == "1"
 _PRIO_HIGHEST = -5  # cudaDeviceGetStreamPriorityRange on H100: [0, -5]; out-of-range values are clamped by the runtime
 _LAYOUTS = {"nchw": 0, "nhwc": 1}
 GRAM_FP64, GRAM_3XTF32 = 0, 1
+# element types of the feature maps the gathers read (CP_F32, CP_BF16, CP_F16 of include/cpb200.h)
+FMAP_DTYPES = {torch.float32: 0, torch.bfloat16: 2, torch.float16: 3}
+
+
+def fmap_dtype_code(dtype):
+    """The C ABI code of a feature-map dtype; TypeError for a type the gathers do not read."""
+    code = FMAP_DTYPES.get(dtype)
+    if code is None:
+        raise TypeError("feature maps must be float32, bfloat16 or float16, got %s" % (dtype,))
+    return code
 
 
 class LassoResult:
@@ -135,7 +145,7 @@ class Engine:
         self._lock = threading.Lock()
         self.launches = 0  # libcpb200 calls issued (each launches >= 1 kernel)
         self._pinned = {}   # (key, shape, dtype) -> page-locked host buffer, allocated once (cudaHostAlloc is slow)
-        self._staging = {}  # (key, shape) -> device staging buffer for maps that are cheaper to DMA whole
+        self._staging = {}  # (key, shape, dtype) -> device staging buffer for maps that are cheaper to DMA whole
         self._xfer = None   # (zero-copy gather stream, DMA stream) of the host-resident input path
         self._aux = None    # (handle, lowest-priority stream) of the deferred full Grams (select_channels_async)
 
@@ -171,11 +181,11 @@ class Engine:
             self._seq = (getattr(self, "_seq", -1) + 1) % 256
             return self._seq
 
-    def staging(self, key, shape):
-        k = (key, tuple(shape))
+    def staging(self, key, shape, dtype=torch.float32):
+        k = (key, tuple(shape), dtype)
         t = self._staging.get(k)
         if t is None:
-            t = self._staging[k] = torch.empty(tuple(shape), dtype=torch.float32, device=self.device)
+            t = self._staging[k] = torch.empty(tuple(shape), dtype=dtype, device=self.device)
         return t
 
     def xfer_streams(self):
@@ -239,9 +249,11 @@ class Engine:
 
     # ------------------------------------------------------------------ kernels
     def patch_gather(self, fmap, randx, randy, B, P, k, pad, stride, relu=True, layout="nchw", out=None):
-        """fmap: (nbatch*B, c, H, W) [nchw] or (nbatch*B, H, W, c) [nhwc] fp32 on device;
-        randx/randy: (nbatch, P) int32 on device.  Returns X (nbatch*P*B, c*k*k) fp32."""
-        assert fmap.dtype == torch.float32 and fmap.is_contiguous()
+        """fmap: (nbatch*B, c, H, W) [nchw] or (nbatch*B, H, W, c) [nhwc], float32 / bfloat16 / float16, on device
+        or (nchw) in pinned host memory; randx/randy: (nbatch, P) int32 on device.  Returns X (nbatch*P*B, c*k*k)
+        fp32 -- 16-bit maps are widened exactly, so X equals the X of fmap.float()."""
+        dt = fmap_dtype_code(fmap.dtype)
+        assert fmap.is_contiguous()
         nimg = fmap.shape[0]
         assert nimg % B == 0
         nbatch = nimg // B
@@ -255,14 +267,16 @@ class Engine:
         if out is None:
             out = self.empty(rows, K, dtype=torch.float32)
         assert out.shape == (rows, K) and out.dtype == torch.float32 and out.stride(1) == 1
-        self._call(self.lib.cp_patch_gather(self.h, self._p(fmap, "const float*"), nbatch, B, c, H, W,
-                                            _LAYOUTS[layout], self._p(randx, "const int32_t*"),
-                                            self._p(randy, "const int32_t*"), P, k, pad, stride, int(bool(relu)),
-                                            self._p(out, "float*"), out.stride(0), self._s()))
+        self._call(self.lib.cp_patch_gather_typed(self.h, self._p(fmap, "const void*"), dt, nbatch, B, c, H, W,
+                                                  _LAYOUTS[layout], self._p(randx, "const int32_t*"),
+                                                  self._p(randy, "const int32_t*"), P, k, pad, stride, int(bool(relu)),
+                                                  self._p(out, "float*"), out.stride(0), self._s()))
         return out
 
     def point_gather(self, fmap, randx, randy, B, P, layout="nchw", out=None):
-        assert fmap.dtype == torch.float32 and fmap.is_contiguous()
+        """Y (nbatch*P*B, n) fp32 at the sampled points of fmap (float32 / bfloat16 / float16, widened exactly)."""
+        dt = fmap_dtype_code(fmap.dtype)
+        assert fmap.is_contiguous()
         nimg = fmap.shape[0]
         nbatch = nimg // B
         if layout == "nchw":
@@ -272,10 +286,10 @@ class Engine:
         rows = nbatch * P * B
         if out is None:
             out = self.empty(rows, n, dtype=torch.float32)
-        self._call(self.lib.cp_point_gather(self.h, self._p(fmap, "const float*"), nbatch, B, n, H, W,
-                                            _LAYOUTS[layout], self._p(randx, "const int32_t*"),
-                                            self._p(randy, "const int32_t*"), P, self._p(out, "float*"),
-                                            out.stride(0), self._s()))
+        self._call(self.lib.cp_point_gather_typed(self.h, self._p(fmap, "const void*"), dt, nbatch, B, n, H, W,
+                                                  _LAYOUTS[layout], self._p(randx, "const int32_t*"),
+                                                  self._p(randy, "const int32_t*"), P, self._p(out, "float*"),
+                                                  out.stride(0), self._s()))
         return out
 
     def gram(self, X, Y=None, y_bias=None, rows=None, want_G=True, want_B=True, want_sums=True, want_yy=False,

@@ -58,10 +58,13 @@ class ConvStackForward:
     reference after ``seperateConvReLU`` (net.py:1228): blob ``<conv>`` holds the PRE-ReLU conv
     output; the next conv's bottom is ``<conv>_relu`` or ``pool<k>`` (post-ReLU).
     ``images_by_batch(batch) -> (B, 3, H, W)`` supplies the un-frozen batches (Caffe's data layer);
-    frozen runs pass the stored images in (net.py:446-447)."""
+    frozen runs pass the stored images in (net.py:446-447).
+    ``dtype``: the type the stack runs in (images and weights are rounded to it; a bfloat16 or float16 forward is
+    what autocast hands over on an H100).  The blobs stay in that type: the gathers read 16-bit maps directly."""
 
-    def __init__(self, images_by_batch=None):
+    def __init__(self, images_by_batch=None, dtype=torch.float32):
         self.images_by_batch = images_by_batch
+        self.dtype = dtype
 
     def data(self, batch):
         return self.images_by_batch(batch)
@@ -69,11 +72,11 @@ class ConvStackForward:
     def __call__(self, net, data, upto=None):
         dev = net.eng.device
         x = data if isinstance(data, torch.Tensor) else torch.as_tensor(np.asarray(data, dtype=np.float32))
-        x = x.to(dev, torch.float32)
+        x = x.to(dev, torch.float32).to(self.dtype)
         blobs = {"data": x}
         for spec in net._specs:
-            w = net._w[spec.name]
-            b = net._b[spec.name]
+            w = net._w[spec.name].to(self.dtype)
+            b = net._b[spec.name].to(self.dtype)
             y = F.conv2d(blobs[spec.bottom], w, b, stride=spec.stride, padding=spec.pad)
             blobs[spec.name] = y
             r = F.relu(y)
@@ -198,6 +201,8 @@ class Net:
                     if batch == 0:
                         points_dict["data"] = tuple(data.shape)       # net.py:432-433
                         points_dict["label"] = (data.shape[0], 1, 1, 1)
+                    if data.dtype == torch.bfloat16:  # numpy has no bfloat16: stored widened (exact)
+                        data = data.float()
                     points_dict[(batch, 0)] = data.cpu().numpy().copy()  # net.py:441-442
                     points_dict[(batch, 1)] = np.zeros((data.shape[0], 1, 1, 1), dtype=np.float32)
             for name in names:

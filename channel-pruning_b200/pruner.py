@@ -104,8 +104,8 @@ class LayerResult:
 
 def prune_layers(eng: Engine, shapes, datas, right0=1e-3, rank_tol=.1, from_host=False, to_host=False, trace=None):
     """Runs the layer problems ``shapes[i]`` / ``datas[i]`` (see synth.make_problem_device) on
-    ``eng``.  from_host: feature maps are taken from pinned host memory (datas[i]['fmap_host'])
-    and copied in the pipeline; to_host: results are copied back to pinned host memory.
+    ``eng``.  from_host: feature maps are taken from pinned host memory (datas[i]['fmap_host'], float32, bfloat16
+    or float16) and copied in the pipeline; to_host: results are copied back to pinned host memory.
     trace: optional dict; filled with {layer name: [(label, timing event), ...]} plus '_t0' (device timeline
     of the step: profiles/e2e_breakdown.py prints it).
     Batch mode: the problems are INDEPENDENT -- every alpha search starts from ``right0`` and the seeds come with the
@@ -135,16 +135,23 @@ def prune_layers(eng: Engine, shapes, datas, right0=1e-3, rank_tol=.1, from_host
 ZC_LINES_PER_S = 2.6e8
 
 
-def zero_copy_lines(s):
-    """128-byte lines the in-place gather touches in host memory (the k rows of a window are W*4 bytes apart)."""
-    row = s.W * 4 if hasattr(s, "W") else 4 * 64
-    lines = min(s.k, -(-((s.k - 1) * row + s.k * 4) // 128) + 1) if s.k > 1 else 1
+def zero_copy_lines(s, esize=4):
+    """128-byte lines the in-place gather touches in host memory (the k rows of a window are W*esize bytes apart;
+    esize: bytes per map element)."""
+    row = s.W * esize if hasattr(s, "W") else esize * 64
+    lines = min(s.k, -(-((s.k - 1) * row + s.k * esize) // 128) + 1) if s.k > 1 else 1
     return s.N * s.c * lines
 
 
-def _zero_copy_seconds(s):
+def _zero_copy_seconds(s, esize=4):
     """Model of the in-place gather over PCIe: it is bound by the number of read requests."""
-    return zero_copy_lines(s) / ZC_LINES_PER_S
+    return zero_copy_lines(s, esize) / ZC_LINES_PER_S
+
+
+def _element_size(fmap):
+    """Bytes per element of a host map (float32 4, bfloat16 / float16 2); a map that only reports numel() counts as
+    float32."""
+    return fmap.element_size() if hasattr(fmap, "element_size") else 4
 
 
 def h2d_plan(shapes, datas, from_host):
@@ -161,9 +168,10 @@ def h2d_plan(shapes, datas, from_host):
     ratio = float(os.environ.get("CPB200_DMA_RATIO", "0.8"))
     plan = []
     for s, d in zip(shapes, datas):
-        nbytes = d["fmap_host"].numel() * 4
+        esize = _element_size(d["fmap_host"])
+        nbytes = d["fmap_host"].numel() * esize
         t_dma = nbytes / 50e9 + 1e-4
-        plan.append("dma" if (nbytes <= cap and t_dma < ratio * _zero_copy_seconds(s)) else "zc")
+        plan.append("dma" if (nbytes <= cap and t_dma < ratio * _zero_copy_seconds(s, esize)) else "zc")
     return plan
 
 
@@ -188,7 +196,7 @@ def _prune_layers_ordered(eng, shapes, datas, right0, rank_tol, from_host, to_ho
                            key=lambda i: (datas[i]["fmap_host"].numel(), i))
         for i in dma_order:
             with torch.cuda.stream(dma_stream):
-                st = eng.staging(("fmap", i), datas[i]["fmap_host"].shape)
+                st = eng.staging(("fmap", i), datas[i]["fmap_host"].shape, datas[i]["fmap_host"].dtype)
                 st.copy_(datas[i]["fmap_host"], non_blocking=True)
                 _mark(trace, shapes[i].name, "dma_done")
                 ev = torch.cuda.Event()
@@ -221,7 +229,7 @@ def _prune_layers_ordered(eng, shapes, datas, right0, rank_tol, from_host, to_ho
                 else:
                     fmap = obj
             elif from_host == "copy":
-                fmap = eng.staging(("fmap", i), d["fmap_host"].shape)
+                fmap = eng.staging(("fmap", i), d["fmap_host"].shape, d["fmap_host"].dtype)
                 fmap.copy_(d["fmap_host"], non_blocking=True)
             elif from_host:
                 # zero-copy: the gather kernel reads the sampled windows straight out of pinned host memory;

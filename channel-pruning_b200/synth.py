@@ -133,13 +133,16 @@ def fmap_nchw(d):
     return d["fmap"].permute(0, 3, 1, 2) if d.get("layout", "nchw") == "nhwc" else d["fmap"]
 
 
-def make_problem_device(shape: LayerShape, seed: int, eng, noise=0.01, pinned_host=False, layout="nchw"):
+def make_problem_device(shape: LayerShape, seed: int, eng, noise=0.01, pinned_host=False, layout="nchw", dtype=None):
     """Device instance (torch CUDA generator), sized for BASELINE configs (GBs of feature maps).
     feats are produced with the library's own gather + a torch fp64 matmul: this is data
     generation, outside any timed region.
     layout: how the bottom blob sits in HBM.  'nhwc' (channels last, what a device-side forward provider hands over)
     takes the TMA gather; the VALUES are those of the 'nchw' instance of the same seed.  The pinned host copy
-    (fmap_host) always keeps the reference's NCHW blob order."""
+    (fmap_host) always keeps the reference's NCHW blob order.
+    dtype: element type of the feature maps (fmap, fmap_host): None / torch.float32, or torch.bfloat16 /
+    torch.float16 as a 16-bit forward pass would hand them over -- drawn in fp32 as for float32, then rounded; the
+    targets are computed from the rounded map."""
     import torch
 
     s = shape
@@ -147,6 +150,8 @@ def make_problem_device(shape: LayerShape, seed: int, eng, noise=0.01, pinned_ho
     g = torch.Generator(device=dev)
     g.manual_seed(seed)
     fmap = torch.randn((s.nbatch * s.B, s.c, s.H, s.W), generator=g, device=dev, dtype=torch.float32)
+    if dtype is not None and dtype != torch.float32:
+        fmap = fmap.to(dtype)
     r = np.random.RandomState(seed)
     randx = torch.as_tensor(r.randint(0, s.Ho, (s.nbatch, s.P)).astype(np.int32), device=dev)
     randy = torch.as_tensor(r.randint(0, s.Ho, (s.nbatch, s.P)).astype(np.int32), device=dev)
@@ -163,7 +168,7 @@ def make_problem_device(shape: LayerShape, seed: int, eng, noise=0.01, pinned_ho
                layout=layout)
     del X, Y
     if pinned_host:
-        out["fmap_host"] = torch.empty(fmap.shape, dtype=torch.float32, pin_memory=True)
+        out["fmap_host"] = torch.empty(fmap.shape, dtype=fmap.dtype, pin_memory=True)
         out["fmap_host"].copy_(fmap)
     if layout == "nhwc":
         out["fmap"] = fmap.permute(0, 2, 3, 1).contiguous()

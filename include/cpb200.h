@@ -45,9 +45,11 @@ enum {
 /* feature-map layouts accepted by the gather kernels */
 enum { CP_LAYOUT_NCHW = 0, CP_LAYOUT_NHWC = 1 };
 
-/* element type of the Y operand (feature maps are fp32; a caller of the Python-level
- * decompose.dictionary may hand over float64 targets, which are then used exactly) */
-enum { CP_F32 = 0, CP_F64 = 1 };
+/* element types.  Y operand of cp_gram and the solvers: CP_F32 or CP_F64 (a caller of the Python-level
+ * decompose.dictionary may hand over float64 targets, which are then used exactly).  Feature map of the gathers
+ * (cp_patch_gather_typed / cp_point_gather_typed): CP_F32, CP_BF16 or CP_F16 -- what a 16-bit forward pass
+ * (autocast, channels_last) produces; the gathered X and Y are fp32 either way, widened exactly. */
+enum { CP_F32 = 0, CP_F64 = 1, CP_BF16 = 2, CP_F16 = 3 };
 
 /* arithmetic of cp_gram */
 enum {
@@ -86,14 +88,19 @@ int cp_gram_kernel_ms(cp_handle_t h, float *ms);
  * Sparse-point im2col -- replaces Net.extract_XY (lib/net.py:534-684, w1=None
  * branch) plus the relu of Net.dictionary_kernel (lib/net.py:1720) when relu != 0.
  *
- *   fmap   : nbatch*B images, layout NCHW (B,c,H,W) or NHWC (B,H,W,c), fp32.  Device memory, or -- NCHW --
+ *   fmap   : nbatch*B images, layout NCHW (B,c,H,W) or NHWC (B,H,W,c), fp32 (cp_patch_gather) or fmap_dtype
+ *            CP_F32 | CP_BF16 | CP_F16 (cp_patch_gather_typed; CP_F64 and other codes return CP_ERR_INVALID).
+ *            16-bit values are widened exactly to fp32 and the relu is applied after widening, so X is bit for
+ *            bit the X of the fp32 map holding the widened values.  Device memory, or -- NCHW --
  *            page-locked host memory mapped under UVA (cudaHostAlloc / pinned torch tensor): the kernel then
  *            reads the sampled windows in place over PCIe with a small persistent grid (the reference keeps
  *            its feature maps in host RAM; only the windows have to cross).
- *            NHWC in device memory with c % 4 == 0, c >= 16 and 16-byte aligned fmap / X_out / ldx takes the TMA
- *            path (csrc/gather_tma.cu): one 4-D tensor-map request per k x k x c window, padding taps zero-filled
+ *            NHWC in device memory with c >= 16, c % 4 == 0 (fp32) or c % 8 == 0 (bf16 / fp16: the 16-byte
+ *            stride rule of TMA), and 16-byte aligned fmap / X_out / ldx takes the TMA path
+ *            (csrc/gather_tma.cu): one 4-D tensor-map request per k x k x c window, padding taps zero-filled
  *            by the copy engine, the patch row leaves as one bulk store -- 74 % of the HBM copy rate at conv4_x
- *            (NCHW: 24 %; k-float runs cannot be fetched at sector efficiency).  Results are bit-identical.
+ *            (NCHW: 24 %; k-float runs cannot be fetched at sector efficiency).  Other NHWC maps take the SIMT
+ *            kernel.  Results are bit-identical.
  *   randx  : nbatch*P sampled output rows   (points_dict[(batch, Y, "randx")])
  *   randy  : nbatch*P sampled output cols
  *   window : rows [stride*x - pad, +k), cols [stride*y - pad, +k) of the bottom
@@ -104,16 +111,23 @@ int cp_gram_kernel_ms(cp_handle_t h, float *ms);
 int cp_patch_gather(cp_handle_t h, const float *fmap, int nbatch, int B, int c, int H, int W, int layout,
                     const int32_t *randx, const int32_t *randy, int P, int k, int pad, int stride, int relu,
                     float *X_out, int64_t ldx, cp_stream_t stream);
+int cp_patch_gather_typed(cp_handle_t h, const void *fmap, int fmap_dtype, int nbatch, int B, int c, int H, int W,
+                          int layout, const int32_t *randx, const int32_t *randy, int P, int k, int pad, int stride,
+                          int relu, float *X_out, int64_t ldx, cp_stream_t stream);
 
 /*
  * Point gather -- replaces the gather of Net.extract_features (lib/net.py:509-519):
  *   Y_out[(batch*P+point)*B + image, j] = fmap[batch*B+image, j, randx, randy].
  * fp32 out (the reference widens to fp64; the bias of lib/net.py:1707 is applied
- * exactly, in fp64, inside cp_gram via y_bias).
+ * exactly, in fp64, inside cp_gram via y_bias).  The map: fp32 (cp_point_gather), or fmap_dtype CP_F32 | CP_BF16 |
+ * CP_F16 (cp_point_gather_typed), widened exactly.
  */
 int cp_point_gather(cp_handle_t h, const float *fmap, int nbatch, int B, int n, int H, int W, int layout,
                     const int32_t *randx, const int32_t *randy, int P, float *Y_out, int64_t ldy,
                     cp_stream_t stream);
+int cp_point_gather_typed(cp_handle_t h, const void *fmap, int fmap_dtype, int nbatch, int B, int n, int H, int W,
+                          int layout, const int32_t *randx, const int32_t *randy, int P, float *Y_out, int64_t ldy,
+                          cp_stream_t stream);
 
 /*
  * Tall-skinny Gram / cross products -- replaces the O(N K^2) arithmetic inside
