@@ -16,8 +16,6 @@
 // Element type of the map: fp32, bf16 or fp16 (template parameter T, fmap_types.cuh).  X and Y are fp32 in every
 // case; the ReLU is applied to the widened value with the fp32 kernel's expression, so -0, inf and NaN come out as the
 // fp32 kernel gives them for the widened map.
-#include <cstdlib>
-
 #include "common.cuh"
 #include "fmap_types.cuh"
 
@@ -124,21 +122,14 @@ bool cp_gather_tma_eligible(const void *fmap, int esize, int c, int k, float *X_
 int cp_patch_gather_tma(cp_handle_t h, const void *fmap, int fmap_dtype, int nbatch, int B, int c, int H, int W,
                         const int32_t *randx, const int32_t *randy, int P, int k, int pad, int stride, int relu,
                         float *X_out, int64_t ldx, cudaStream_t stream);
-static bool tma_enabled() {  // CPB200_GATHER_TMA=0 keeps the SIMT kernel (A/B measurements)
-    static const bool on = [] {
-        const char *e = getenv("CPB200_GATHER_TMA");
-        return !(e && e[0] == '0');
-    }();
-    return on;
-}
 
 template <typename T>
-static void launch_patch_gather_simt(const T *fmap, int layout, bool host_src, int64_t host_ctas, int64_t rows,
+static void launch_patch_gather_simt(const T *fmap, int layout, bool host_src, int64_t rows,
                                      int B, int c, int H, int W, const int32_t *randx, const int32_t *randy, int P,
                                      int k, int pad, int stride, int relu, float *X_out, int64_t ldx,
                                      cudaStream_t stream) {
     if (layout == CP_LAYOUT_NCHW) {
-        const int64_t ncta = host_src ? (rows < host_ctas ? rows : host_ctas) : rows;
+        const int64_t ncta = host_src ? (rows < CP_HOST_GATHER_CTAS ? rows : CP_HOST_GATHER_CTAS) : rows;
         dim3 grid((unsigned)ncta);
         if (k == 3)
             patch_gather_nchw<3><<<grid, 256, 0, stream>>>(fmap, randx, randy, X_out, ldx, rows, B, c, H, W, P, k, pad, stride, relu);
@@ -169,19 +160,12 @@ extern "C" int cp_patch_gather_typed(cp_handle_t h, const void *fmap, int fmap_d
     if (rows == 0) return CP_OK;
     CP_REQUIRE(rows < (1ll << 31), "cp_patch_gather: too many rows");
     bool host_src = false;
-    int64_t host_ctas = CP_HOST_GATHER_CTAS;
     if (layout == CP_LAYOUT_NCHW) {
         // map in (pinned, UVA-mapped) host memory?  then the kernel is a PCIe reader: keep its footprint small
         cudaPointerAttributes pa;
         host_src = cudaPointerGetAttributes(&pa, fmap) == cudaSuccess && pa.type == cudaMemoryTypeHost;
         (void)cudaGetLastError();
-        static const int64_t env_host_ctas = [] {
-            const char *e = getenv("CPB200_HOST_GATHER_CTAS");  // tuning knob (profiles/e2e_breakdown.py)
-            const long v = e ? atol(e) : 0;
-            return (int64_t)(v > 0 ? v : CP_HOST_GATHER_CTAS);
-        }();
-        host_ctas = env_host_ctas;
-    } else if (tma_enabled() && cp_gather_tma_eligible(fmap, esize, c, k, X_out, ldx)) {
+    } else if (cp_gather_tma_eligible(fmap, esize, c, k, X_out, ldx)) {
         // NHWC map in HBM: whole windows by TMA, rows out by bulk store (gather_tma.cu)
         return cp_patch_gather_tma(h, fmap, fmap_dtype, nbatch, B, c, H, W, randx, randy, P, k, pad, stride, relu,
                                    X_out, ldx, stream);
@@ -190,14 +174,14 @@ extern "C" int cp_patch_gather_typed(cp_handle_t h, const void *fmap, int fmap_d
         CP_REQUIRE(smem <= 48 * 1024, "cp_patch_gather: kernel_size %d too large for the NHWC tile", k);
     }
     if (fmap_dtype == CP_F32)
-        launch_patch_gather_simt((const float *)fmap, layout, host_src, host_ctas, rows, B, c, H, W, randx, randy, P,
-                                 k, pad, stride, relu, X_out, ldx, stream);
+        launch_patch_gather_simt((const float *)fmap, layout, host_src, rows, B, c, H, W, randx, randy, P, k, pad,
+                                 stride, relu, X_out, ldx, stream);
     else if (fmap_dtype == CP_BF16)
-        launch_patch_gather_simt((const __nv_bfloat16 *)fmap, layout, host_src, host_ctas, rows, B, c, H, W, randx,
-                                 randy, P, k, pad, stride, relu, X_out, ldx, stream);
+        launch_patch_gather_simt((const __nv_bfloat16 *)fmap, layout, host_src, rows, B, c, H, W, randx, randy, P, k,
+                                 pad, stride, relu, X_out, ldx, stream);
     else
-        launch_patch_gather_simt((const __half *)fmap, layout, host_src, host_ctas, rows, B, c, H, W, randx, randy, P,
-                                 k, pad, stride, relu, X_out, ldx, stream);
+        launch_patch_gather_simt((const __half *)fmap, layout, host_src, rows, B, c, H, W, randx, randy, P, k, pad,
+                                 stride, relu, X_out, ldx, stream);
     CP_CHECK_LAUNCH();
     return CP_OK;
 }

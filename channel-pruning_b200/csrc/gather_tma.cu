@@ -19,8 +19,6 @@
 // The 16-byte rules of TMA (global strides, box rows) then need c % 8 == 0.
 #include <cuda.h>
 
-#include <cstdlib>
-
 #include "common.cuh"
 #include "fmap_types.cuh"
 
@@ -259,12 +257,8 @@ int cp_patch_gather_tma(cp_handle_t h, const void *fmap, int fmap_dtype, int nba
     const size_t budget = 216 * 1024;
     int per_sm = (int)(budget / (2 * row + GT_OUT * out_b + 1024));
     per_sm = per_sm < 1 ? 1 : (per_sm > 4 ? 4 : per_sm);
-    static const int env_per_sm = [] { const char *e = getenv("CPB200_GATHER_CTAS_PER_SM"); return e ? atoi(e) : 0; }();
-    static const int env_stages = [] { const char *e = getenv("CPB200_GATHER_STAGES"); return e ? atoi(e) : 0; }();
-    if (env_per_sm > 0 && env_per_sm < per_sm) per_sm = env_per_sm;  // tuning knobs
     int nstage = (int)((budget / per_sm - 1024 - GT_OUT * out_b) / row);
     if (nstage > 6) nstage = 6;
-    if (env_stages >= 2 && env_stages < nstage) nstage = env_stages;
     Pm.nstage = nstage;
     Pm.box_f = (int)(box_b / esize); Pm.stage_f = (int)(row / esize); Pm.out_f = (int)(out_b / 4);
     const size_t smem = (size_t)nstage * row + GT_OUT * out_b + 2 * nstage * 8 + 256;

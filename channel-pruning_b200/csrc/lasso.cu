@@ -104,36 +104,23 @@ struct SelectParams {
 };
 
 constexpr int MAXC = 2048;   // largest channel count (shared-memory bound)
-#ifndef CP_LASSO_LAG
-#define CP_LASSO_LAG 4
-#endif
-constexpr int LAG = CP_LASSO_LAG;  // deltas the chain warp applies itself (slack of the update warps), 1..5
-static_assert(LAG == 4, "the unrolled chain / update blocks are laid out for LAG = 4 (delta ring static across 16-step "
-                        "blocks, publish targets inside two 16-byte index loads)");
+// Deltas the chain warp applies itself (slack of the update warps).  The unrolled chain / update blocks are laid out for
+// LAG = 4: the delta ring is static across 16-step blocks and the publish targets sit inside two 16-byte index loads.
+constexpr int LAG = 4;
 constexpr int NBULK = 4;     // pair-update warps
 // Role of a warp inside a sweep.  The chain warp sits on warp CHAIN_W: with 7 warps on 4 scheduler partitions, warp 3
 // is the only one that has a partition to itself (0/4, 1/5, 2/6 share), so the serial recurrence never competes for
 // issue slots with a polling warp.  Roles of the others, in warp order: NBULK update warps, packager, sequencer.
-#ifndef CP_LASSO_CHAIN_WARP
-#define CP_LASSO_CHAIN_WARP 3
-#endif
+constexpr int CHAIN_W = 3;
 // Polling back-off (ns) of the warps that wait for the chain: a tight LDS polling loop of five warps keeps the
 // shared-memory pipe busy and lengthens every shared-memory access of the chain warp.
-#ifndef CP_LASSO_SLEEP
-#define CP_LASSO_SLEEP 32
-#endif
-constexpr int CHAIN_W = CP_LASSO_CHAIN_WARP;
+constexpr int POLL_SLEEP_NS = 32;
 constexpr int WS_THREADS = 32 * (3 + NBULK);
 __device__ __forceinline__ int role_of(int warp) {  // -1 chain, 0..NBULK-1 update, NBULK packager, NBULK+1 sequencer
     return warp == CHAIN_W ? -1 : (warp < CHAIN_W ? warp : warp - 1);
 }
-__device__ __forceinline__ void poll_backoff() {
-#if CP_LASSO_SLEEP > 0
-    __nanosleep(CP_LASSO_SLEEP);
-#endif
-}
+__device__ __forceinline__ void poll_backoff() { __nanosleep(POLL_SLEEP_NS); }
 constexpr int QR = 64;       // rings of per-step scalars (steps in flight << QR)
-template <int NPB> struct RingDepth { static constexpr int value = 0; };  // no shared-memory row ring any more (register ring)
 
 __device__ __forceinline__ uint32_t xorshift_step(uint32_t s) {  // sklearn/utils/_random.pxd:20-34 (state update)
     if (s == 0) s = 1;
@@ -247,15 +234,13 @@ template <int NPB>  // pairs per update lane; padded channel count CP = 2 * 32 *
 __global__ void __launch_bounds__(WS_THREADS, 1) lasso_select_kernel(const SelectParams P) {
     constexpr int BL = 32 * NBULK;  // update lanes
     constexpr int CP = 2 * BL * NPB;
-    constexpr int RING = RingDepth<NPB>::value;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int c = P.c, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     double *w = reinterpret_cast<double *>(smem_raw);  // [CP]
     double *Qw = w + CP;
     double *qv = Qw + CP;
     double *dg = qv + CP;
-    double *ring = dg + CP;                 // [RING][CP]
-    double *pk = ring + (size_t)RING * CP;  // [QR][8]: q, Qjj, 1/Qjj, r1 .. r5
+    double *pk = dg + CP;                   // [QR][8]: q, Qjj, 1/Qjj, r1 .. r5
     double *dq = pk + QR * 8;               // [QR][2] published {delta, tag}
     double *xq = dq + QR * 2;               // [QR][2] published {Qw entry, tag}
     uint32_t *active = reinterpret_cast<uint32_t *>(xq + QR * 2);
@@ -276,8 +261,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) lasso_select_kernel(const Selec
         active[e] = e;
         excluded[e] = 0;
     }
-    for (int e = tid; e < RING * CP; e += WS_THREADS) ring[e] = 0.0;  // padding pairs stay zero
-    for (int e = tid; e < QR * 4; e += WS_THREADS) dq[e] = 0.0;        // dq and xq: no tag matches {0, 0}
+    for (int e = tid; e < QR * 4; e += WS_THREADS) dq[e] = 0.0;  // dq and xq: no tag matches {0, 0}
     __syncthreads();
     uint32_t sweep_no = 1;  // tags are (sweep_no << 12) | (step + 1): unique over the whole launch (< 2^20 sweeps)
 
@@ -715,8 +699,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) lasso_select_kernel(const Selec
 template <int NPB>
 int launch_select(const SelectParams &P, cudaStream_t stream) {
     constexpr int CP = 2 * 32 * NBULK * NPB;
-    constexpr int RING = RingDepth<NPB>::value;
-    const size_t smem = (size_t)CP * (4 + RING) * sizeof(double) + (size_t)QR * 12 * sizeof(double) +
+    const size_t smem = (size_t)CP * 4 * sizeof(double) + (size_t)QR * 12 * sizeof(double) +
                         (size_t)CP * (4 * sizeof(uint32_t) + 1) + 16;
     static cp_per_device_flag configured;  // per instantiation, per device
     if (bool *done = configured.slot(); !*done) {

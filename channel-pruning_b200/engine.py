@@ -26,21 +26,9 @@ MAX_PROBES = 64
 # conditioning of the system (profiles/conditioning_map.py maps the weight error against the pivot ratio), so every such solve is followed by ONE step of iterative refinement against the
 # same factor with the residual taken from the data (engine.ls_refine) -- which squares the error -- and is accepted
 # only while the smallest Cholesky pivot keeps at least LS_RATIO_MIN of its original diagonal entry (1 - R^2 of the
-# most collinear column); below that the layer is re-solved from exact-product fp64 statistics.
-LS_RATIO_MIN = float(os.environ.get("CPB200_LS_RATIO_MIN", "0.005"))
-LS_REFINE = os.environ.get("CPB200_LS_REFINE", "1") == "1"
-# Prediction X W' of the refinement residual: "fp64" (SIMT fp64 GEMM), "tc" (tensor cores, through cp_gram on the
-# transposed patches) or "auto" (tensor cores for N >= 20000 only).  The tensor-core Gram (gram_tc2.cu) is one short
-# persistent launch, and the FP64 pipe is the step's scarce resource: "tc" takes 2NK'n flop per layer off it.
-# Default "tc" (in the tensor-core mode).
-LS_RESID = os.environ.get("CPB200_LS_RESID", "tc")
-LS_RESID_TC_MIN_N = 20000
-# Bulk products of the Cholesky solve on the tensor cores when the statistics came from there (cp_ls_tensor_cores)
-LS_TC = os.environ.get("CPB200_LS_TC", "1") == "1"
-# Full Gram of a layer enqueued after its channel search, on a lowest-priority stream (select_channels_async)
-DEFER_FULL_GRAM = os.environ.get("CPB200_DEFER_GRAM", "1") == "1"
+# most collinear column); below that the layer is re-solved from exact-product fp64 statistics (settle_ls).
+LS_RATIO_MIN = 0.005
 
-_PRIO_HIGHEST = -5  # cudaDeviceGetStreamPriorityRange on H100: [0, -5]; out-of-range values are clamped by the runtime
 _LAYOUTS = {"nchw": 0, "nhwc": 1}
 GRAM_FP64, GRAM_3XTF32 = 0, 1
 # element types of the feature maps the gathers read (CP_F32, CP_BF16, CP_F16 of include/cpb200.h)
@@ -120,7 +108,7 @@ class Engine:
         if device is None:
             device = torch.cuda.current_device()
         self.device = torch.device("cuda", device if isinstance(device, int) else torch.device(device).index or 0)
-        if gram_mode is None:  # tensor cores by default; CPB200_GRAM=fp64 selects the exact-product DFMA mode
+        if gram_mode is None:  # tensor cores by default; CPB200_GRAM=fp64 selects the exact-product DMMA mode
             gram_mode = GRAM_FP64 if os.environ.get("CPB200_GRAM", "tc").lower() == "fp64" else GRAM_3XTF32
         self.gram_mode = gram_mode
         self._handles = []
@@ -130,16 +118,10 @@ class Engine:
                 hp = self.ffi.new("cp_handle_t*")
                 _cabi.check(self.lib.cp_create(hp, self.device.index))
                 self._handles.append(hp[0])
-                # The pipeline hands its most expensive problems to the first slots.  CPB200_STREAM_PRIORITY:
-                #   "1"      (default) two levels: the first half of the slots high
-                #   "graded" one level per slot from the highest down (H100: -5 .. 0)        "0"  none
-                # priorities only order CTAs that are not yet resident, so they matter little when the step is bound
-                # by FP64 throughput
-                pol = os.environ.get("CPB200_STREAM_PRIORITY", "1")
-                if pol == "graded":
-                    prio = min(0, _PRIO_HIGHEST + i)
-                else:
-                    prio = -2 if (i < nstreams // 2 and pol == "1") else -1  # 0 is left to the deferred-Gram stream
+                # The pipeline hands its most expensive problems to the first slots: the first half of the slots runs
+                # one level higher.  Priorities only order CTAs that are not yet resident, so they matter little when
+                # the step is bound by FP64 throughput.
+                prio = -2 if i < nstreams // 2 else -1  # 0 is left to the deferred-Gram stream
                 self.streams.append(torch.cuda.Stream(self.device, priority=prio) if nstreams > 1 else None)
         self._tls = threading.local()   # current (handle, stream) slot of each host thread (use_slot)
         self._lock = threading.Lock()
@@ -407,7 +389,7 @@ class Engine:
         b = self.empty(n)
         info = torch.zeros(1, dtype=torch.int32, device=self.device)
         stat = self.empty(1)
-        self.ls_tensor_cores(LS_TC and g.get("mode", GRAM_FP64) != GRAM_FP64)
+        self.ls_tensor_cores(g.get("mode", GRAM_FP64) != GRAM_FP64)
         self._call(self.lib.cp_ls_solve(self.h, self._p(g["G"], "const double*"), self._p(g["B"], "const double*"),
                                         self._p(g["sx"], "const double*"), self._p(g["sy"], "const double*"),
                                         g["N"], g["K"], n, self._p(sel_cols, "const int32_t*"), Ks,
@@ -437,7 +419,7 @@ class Engine:
         Ks = sel_cols.numel() if sel_cols is not None else g["K"]
         info = torch.zeros(1, dtype=torch.int32, device=self.device)
         stat = self.empty(1)
-        self.ls_tensor_cores(LS_TC and g.get("mode", GRAM_FP64) != GRAM_FP64)
+        self.ls_tensor_cores(g.get("mode", GRAM_FP64) != GRAM_FP64)
         self._call(self.lib.cp_ls_factor(self.h, self._p(g["G"], "const double*"), self._p(g["sx"], "const double*"),
                                          g["N"], g["K"], self._p(sel_cols, "const int32_t*"), Ks,
                                          self._p(info, "int32_t*"), self._p(stat, "double*"), self._s()))
@@ -474,10 +456,11 @@ class Engine:
 
     def ls_refine(self, g, X, Y, y_bias, sel_cols, W, b):
         """One step of iterative refinement of (W, b) against the factor the last ls_solve left on this handle:
-        residual from the data (exact fp64), its cross products with X on the tensor cores, forward/backward
-        substitution, correction added in place.  Removes the error tensor-core statistics put into the solution."""
-        tc = LS_RESID == "tc" or (LS_RESID == "auto" and X.shape[0] >= LS_RESID_TC_MIN_N)
-        R = self.ls_residual(X, Y, y_bias, sel_cols, W, b, mode=g["mode"] if tc else GRAM_FP64)
+        residual from the data, its cross products with X on the tensor cores, forward/backward substitution,
+        correction added in place.  Removes the error tensor-core statistics put into the solution.  The prediction
+        X W' of the residual runs in the statistics' mode: on the tensor cores it is one short persistent launch, and
+        it takes 2NK'n flop per layer off the FP64 pipe, the step's scarce resource."""
+        R = self.ls_residual(X, Y, y_bias, sel_cols, W, b, mode=g["mode"])
         gr = self.gram(X, R, want_G=False, mode=g["mode"])
         self.ls_resolve(gr["B"], g["sx"], gr["sy"], sel_cols, accumulate_into=(W, b))
         return W, b
@@ -611,7 +594,7 @@ class Engine:
         # reconstruction.  In the pipeline (one stream per layer) it is therefore enqueued AFTER the search, on a
         # lowest-priority stream with its own handle: the full-GPU launch no longer delays the start of this and of
         # every later layer's single-SM search, it runs in their shadow.
-        defer = DEFER_FULL_GRAM and self.streams[0] is not None
+        defer = self.streams[0] is not None
         if defer:
             cur = torch.cuda.current_stream(self.device)
             ev_x = torch.cuda.Event()
@@ -654,9 +637,9 @@ class Engine:
         if g_full.get("ready") is not None:  # full Gram enqueued on the deferred-Gram stream
             torch.cuda.current_stream(self.device).wait_event(g_full["ready"])
         cols_d = self._cols_device(idxs_host, k2, g_full["K"])
-        if g_full["N"] - 1 >= cols_d.numel():
+        if not ls_dual(g_full["N"], idxs_host, k2):
             W, b, info, stat = self.ls_solve(g_full, cols_d)
-            if g_full["mode"] != GRAM_FP64 and LS_REFINE:
+            if g_full["mode"] != GRAM_FP64:
                 # statistics from the 3xTF32 Gram carry ~4e-7 relative error, which the conditioning of a wide layer
                 # amplifies by orders of magnitude in W and more in b: one refinement step against
                 # the same factor, with the residual taken from the data, restores fp64-level accuracy
@@ -691,15 +674,40 @@ class Engine:
         b = ym - self.mm(W, xm[:, None].contiguous())[:, 0]
         return W, b, int(keep.sum().item())
 
-    @staticmethod
-    def ls_verdict(info, stat, mode, dual=False):
-        """'ok' | 'redo' (tensor-core statistics too inaccurate for this conditioning: re-solve in fp64) |
-        'singular' (a pivot fell below sklearn's rank cut-off even with exact statistics)."""
-        if mode == GRAM_FP64 or dual:
-            return "singular" if info else "ok"
-        if info or not (stat >= LS_RATIO_MIN):
-            return "redo"
-        return "ok"
+
+def ls_dual(N, idxs_host, k2):
+    """True when the K' = kept channels * k2 selected columns leave fewer than K' degrees of freedom in the N centred
+    rows: the normal equations are singular by construction, so the solve works on the data (cp_ls_solve_dual)."""
+    return N - 1 < int(np.count_nonzero(idxs_host)) * k2
+
+
+def settle_ls(eng, X, Y, y_bias, idxs_host, k2, mode, fail, ratio):
+    """Acceptance policy of a reconstruct_async solve, given its Cholesky status ``fail`` and pivot ratio ``ratio``
+    (read back on the host), in statistics mode ``mode``.  Work it adds runs on the current stream.
+      - fp64 statistics or the dual path: accepted unless the Cholesky failed ('singular').
+      - tensor-core statistics: accepted while the Cholesky succeeded and ratio >= LS_RATIO_MIN (NaN fails);
+        otherwise re-solved from exact-product fp64 statistics ('redo->ok', or singular when that fails too).
+      - singular (a pivot below 1e-12 of its diagonal, even with exact statistics): numerically rank deficient.  The
+        reference's gelsd drops singular values below 1e-6 sigma_max (cond=1e-6, sklearn _base.py:752) and returns
+        the minimum-norm solution; reconstruct_truncated applies that rule through the SVD of the data: 'truncated',
+        with the rank it kept.
+    Returns (W, b, record): W and b replace the first solve's, or are None when it stands; record holds
+    pivot_ratio, verdict ('ok' | 'redo->ok' | 'truncated') and, where they apply, pivot_ratio_exact and rank."""
+    rec = {"pivot_ratio": ratio}
+    if mode == GRAM_FP64 or ls_dual(X.shape[0], idxs_host, k2):
+        verdict = "singular" if fail else "ok"
+    else:
+        verdict = "redo" if fail or not (ratio >= LS_RATIO_MIN) else "ok"
+    W = b = None
+    if verdict == "redo":
+        W, b, info, stat = eng.reconstruct_exact_async(X, Y, y_bias, idxs_host, k2)
+        fail, rec["pivot_ratio_exact"] = int(info.cpu()[0]), float(stat.cpu()[0])
+        verdict = "singular" if fail else "redo->ok"
+    if verdict == "singular":
+        W, b, rec["rank"] = eng.reconstruct_truncated(X, Y, y_bias, idxs_host, k2)
+        verdict = "truncated"
+    rec["verdict"] = verdict
+    return W, b, rec
 
 
 def window(rank, rank_tol):

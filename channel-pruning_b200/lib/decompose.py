@@ -19,7 +19,7 @@ import torch
 
 from . import cfgs
 from .cfgs import c as dcfgs
-from ..engine import MAX_PROBES, RAND_R_MAX, get_engine
+from ..engine import MAX_PROBES, RAND_R_MAX, get_engine, settle_ls
 
 
 def relu(x):
@@ -143,29 +143,13 @@ def _dictionary_device(eng, Xd, W2m, Yd, y_bias, c, h, rank, alpha=1e-4):
 
 
 def _solve_ls(eng, g_full, Xd, Yd, y_bias, idxs, k2, info=None):
-    """LS on the surviving channels with the conditioning policy of engine.LS_RATIO_MIN: statistics from the
-    tensor-core Gram are used while the Cholesky stays well conditioned, otherwise the layer is re-solved from
-    exact-product fp64 statistics; a pivot below sklearn's rank cut-off (cond=1e-6, _base.py:752) switches to the
-    truncated minimum-norm solve gelsd would return."""
+    """LS on the surviving channels, accepted or redone by the conditioning policy of engine.settle_ls."""
     Wd, bd, info_d, stat_d = eng.reconstruct_async(g_full, Xd, Yd, y_bias, idxs, k2)
-    dual = not (g_full["N"] - 1 >= int(np.count_nonzero(idxs)) * k2)
     fail, ratio = int(info_d.cpu()[0]), float(stat_d.cpu()[0])
-    verdict = eng.ls_verdict(fail, ratio, g_full["mode"], dual)
+    W, b, rec = settle_ls(eng, Xd, Yd, y_bias, idxs, k2, g_full["mode"], fail, ratio)
     if info is not None:
-        info["ls"] = {"pivot_ratio": ratio, "verdict": verdict}
-    if verdict == "redo":
-        Wd, bd, info_d, stat_d = eng.reconstruct_exact_async(Xd, Yd, y_bias, idxs, k2)
-        fail, ratio = int(info_d.cpu()[0]), float(stat_d.cpu()[0])
-        verdict = "singular" if fail else "ok"
-        if info is not None:
-            info["ls"].update(pivot_ratio_exact=ratio, verdict="redo->" + verdict)
-    if verdict == "singular":
-        # numerically rank deficient (a pivot below 1e-12 of its diagonal): the reference's gelsd truncates singular
-        # values below 1e-6 sigma_max and returns the minimum-norm solution -- same rule, through the SVD of the data
-        Wd, bd, kept = eng.reconstruct_truncated(Xd, Yd, y_bias, idxs, k2)
-        if info is not None:
-            info["ls"].update(verdict="truncated", rank=kept)
-    return Wd, bd
+        info["ls"] = rec
+    return (Wd, bd) if W is None else (W, b)
 
 
 def fc_kernel(X, Y, copy_X=True, W=None, B=None, ret_reg=False, fit_intercept=True):

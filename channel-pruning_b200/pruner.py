@@ -18,12 +18,12 @@ import time
 import numpy as np
 import torch
 
-from .engine import Engine, window
+from .engine import Engine, ls_dual, settle_ls, window
 
 
 # ---------------------------------------------------------------------------- assignment
-# host threads that issue the reconstructions of phase 2 (CPB200_PHASE2_THREADS=1: the single-threaded polling loop)
-PHASE2_THREADS = int(os.environ.get("CPB200_PHASE2_THREADS", "6"))
+# host threads that issue the reconstructions of phase 2 (an engine with one stream uses the single-threaded loop)
+PHASE2_THREADS = 6
 _POOLS = {}
 
 
@@ -292,7 +292,7 @@ def _prune_layers_ordered(eng, shapes, datas, right0, rank_tol, from_host, to_ho
             ev_ls.record()
             _mark(trace, s.name, "ls_done")
         r.probes = res
-        r.info = {"mode": g_full["mode"], "dual": not (g_full["N"] - 1 >= int(r.idxs.sum()) * s.k * s.k)}
+        r.info = {"mode": g_full["mode"], "dual": ls_dual(g_full["N"], r.idxs, s.k * s.k)}
         out[i] = r
         return (i, chk, ev_ls)
 
@@ -312,33 +312,18 @@ def _prune_layers_ordered(eng, shapes, datas, right0, rank_tol, from_host, to_ho
         else:
             checks.append(reconstruct_layer(i))
     checks.extend(f.result() for f in futures)
-    # ---- every reconstruction is CHECKED before it is handed out: Cholesky status + conditioning signal.
-    # Tensor-core statistics are accepted only for well-conditioned systems (engine.LS_RATIO_MIN); otherwise the
-    # layer is re-solved from exact-product fp64 statistics; a system that is rank deficient by sklearn's cut-off
-    # gets the truncated minimum-norm solution the reference's gelsd returns.
+    # ---- every reconstruction is CHECKED before it is handed out (Cholesky status + conditioning signal) and, where
+    # the policy says so, redone on its layer's slot (engine.settle_ls).
     for i, chk, ev_ls in checks:
         ev_ls.synchronize()
         s, d, r = shapes[i], datas[i], out[i]
-        fail, ratio = int(chk[0][0]), float(chk[1][0])
-        verdict = eng.ls_verdict(fail, ratio, r.info["mode"], r.info["dual"])
-        r.info.update(pivot_ratio=ratio, verdict=verdict)
-        if verdict == "redo":
-            stream = eng.use_slot(i)
-            ctx = torch.cuda.stream(stream) if stream is not None else _null()
-            with ctx:
-                X = phase1[i][0]
-                W, b, info, stat = eng.reconstruct_exact_async(X, d["feats"], d["b2"], r.idxs, s.k * s.k)
-                fail, ratio = int(info.cpu()[0]), float(stat.cpu()[0])
+        stream = eng.use_slot(i)
+        with torch.cuda.stream(stream) if stream is not None else _null():
+            W, b, rec = settle_ls(eng, phase1[i][0], d["feats"], d["b2"], r.idxs, s.k * s.k, r.info["mode"],
+                                  int(chk[0][0]), float(chk[1][0]))
+            if W is not None:
                 r.W, r.b = _maybe_to_host(eng, i, W, b, to_host)
-            verdict = "singular" if fail else "ok"
-            r.info.update(pivot_ratio_exact=ratio, verdict="redo->" + verdict)
-        if verdict == "singular":  # gelsd's truncated minimum-norm solution (slow path, see Engine.reconstruct_truncated)
-            stream = eng.use_slot(i)
-            ctx = torch.cuda.stream(stream) if stream is not None else _null()
-            with ctx:
-                W, b, kept = eng.reconstruct_truncated(phase1[i][0], d["feats"], d["b2"], r.idxs, s.k * s.k)
-                r.W, r.b = _maybe_to_host(eng, i, W, b, to_host)
-            r.info.update(verdict="truncated", rank=kept)
+        r.info.update(rec)
     for st in eng.streams:
         if st is not None:
             main.wait_stream(st)
