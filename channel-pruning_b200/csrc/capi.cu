@@ -23,44 +23,21 @@ extern "C" int cp_create(cp_handle_t *out, int device) {
     cp_handle_s *h = new cp_handle_s();
     h->device = device;
     h->num_sms = prop.multiProcessorCount;
-    h->ws = nullptr;
-    h->ws_bytes = 0;
-    h->tmap_encode = nullptr;
-    h->side = nullptr;
-    h->bulk = nullptr;
-    h->ev_panel = nullptr;
-    h->ev_side = nullptr;
-    h->ev_bulk = nullptr;
-    h->potrf_configured = false;
-    h->fac = nullptr;
-    h->fac_bytes = 0;
-    h->fac_K = h->fac_Kfull = 0;
-    h->fac_N = 0;
-    h->fac_rows = 0;
-    h->aux = nullptr;
-    h->aux_bytes = 0;
-    h->gram_profile = false;
-    h->ev_gram0 = h->ev_gram1 = nullptr;
-    h->ls_tc = false;
-    for (int i = 0; i < 3; ++i) {
-        h->tcbuf[i] = nullptr;
-        h->tcbuf_bytes[i] = 0;
-    }
     *out = h;
     return CP_OK;
 }
 
 extern "C" int cp_destroy(cp_handle_t h) {
     if (!h) return CP_OK;
-    if (h->ws || h->side || h->fac || h->aux || h->ev_gram0 || h->tcbuf[0] || h->tcbuf[1] || h->tcbuf[2]) {
+    cp_buffer *bufs[] = {&h->ws, &h->aux, &h->fac.buf, &h->tcbuf[0], &h->tcbuf[1], &h->tcbuf[2]};
+    bool held = h->side || h->ev_gram0;
+    for (cp_buffer *b : bufs) held = held || b->ptr;
+    if (held) {
         int cur = 0;
         cudaGetDevice(&cur);
         cudaSetDevice(h->device);
-        if (h->ws) cudaFree(h->ws);
-        if (h->fac) cudaFree(h->fac);
-        if (h->aux) cudaFree(h->aux);
-        for (int i = 0; i < 3; ++i)
-            if (h->tcbuf[i]) cudaFree(h->tcbuf[i]);
+        for (cp_buffer *b : bufs)
+            if (b->ptr) cudaFree(b->ptr);
         if (h->ev_gram0) {
             cudaEventDestroy(h->ev_gram0);
             cudaEventDestroy(h->ev_gram1);
@@ -104,39 +81,32 @@ extern "C" int cp_gram_kernel_ms(cp_handle_t h, float *ms) {
     return CP_OK;
 }
 
-extern "C" int64_t cp_workspace_bytes(cp_handle_t h) { return h ? (int64_t)h->ws_bytes : 0; }
+extern "C" int64_t cp_workspace_bytes(cp_handle_t h) { return h ? (int64_t)h->ws.bytes : 0; }
+
+int cp_buffer_reserve(cp_buffer &buf, size_t need, size_t slack_div, const char *what) {
+    if (need <= buf.bytes) return CP_OK;
+    if (buf.ptr) CP_CUDA(cudaFree(buf.ptr));
+    buf = {};
+    const size_t want = cp_align_up(need + need / slack_div, (size_t)1 << 20);
+    cudaError_t e = cudaMalloc(&buf.ptr, want);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        CP_FAIL(CP_ERR_WORKSPACE, "%s of %zu bytes failed: %s", what, want, cudaGetErrorString(e));
+    }
+    buf.bytes = want;
+    return CP_OK;
+}
 
 int cp_ws_reserve(cp_handle_t h, size_t bytes, void **out) {
-    if (bytes > h->ws_bytes) {
-        // cudaFree synchronises the device, so no in-flight kernel can still be using the old block
-        if (h->ws) CP_CUDA(cudaFree(h->ws));
-        h->ws = nullptr;
-        h->ws_bytes = 0;
-        size_t want = cp_align_up(bytes + bytes / 8, (size_t)1 << 20);
-        cudaError_t e = cudaMalloc(&h->ws, want);
-        if (e != cudaSuccess) {
-            cudaGetLastError();
-            CP_FAIL(CP_ERR_WORKSPACE, "workspace allocation of %zu bytes failed: %s", want, cudaGetErrorString(e));
-        }
-        h->ws_bytes = want;
-    }
-    *out = h->ws;
+    int rc = cp_buffer_reserve(h->ws, bytes, 8, "workspace allocation");
+    if (rc) return rc;
+    *out = h->ws.ptr;
     return CP_OK;
 }
 
 int cp_aux_reserve(cp_handle_t h, size_t bytes, void **out) {
-    if (bytes > h->aux_bytes) {
-        if (h->aux) CP_CUDA(cudaFree(h->aux));
-        h->aux = nullptr;
-        h->aux_bytes = 0;
-        size_t want = cp_align_up(bytes + bytes / 8, (size_t)1 << 20);
-        cudaError_t e = cudaMalloc(&h->aux, want);
-        if (e != cudaSuccess) {
-            cudaGetLastError();
-            CP_FAIL(CP_ERR_WORKSPACE, "auxiliary workspace allocation of %zu bytes failed: %s", want, cudaGetErrorString(e));
-        }
-        h->aux_bytes = want;
-    }
-    *out = h->aux;
+    int rc = cp_buffer_reserve(h->aux, bytes, 8, "auxiliary workspace allocation");
+    if (rc) return rc;
+    *out = h->aux.ptr;
     return CP_OK;
 }

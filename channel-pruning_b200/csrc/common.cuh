@@ -7,35 +7,47 @@
 
 #include "../../include/cpb200.h"
 
+// A device allocation of the handle, grown on demand by cp_buffer_reserve.
+struct cp_buffer {
+    void *ptr;
+    size_t bytes;
+};
+
+// Makes `buf` hold at least `need` bytes.  A larger block replaces the old one (cudaFree synchronises the device, so no
+// kernel in flight still uses it), with need / slack_div bytes of slack, rounded up to 1 MiB.  `what` starts the error
+// message.
+int cp_buffer_reserve(cp_buffer &buf, size_t need, size_t slack_div, const char *what);
+
+// The Cholesky factor kept between cp_ls_factor / cp_ls_solve and cp_ls_resolve (ls.cu).  It has its own allocation
+// because every entry point reuses the scratch `ws`.
+struct cp_kept_factor {
+    cp_buffer buf;
+    int K, Kfull;  // K == 0: the handle holds no factor
+    int64_t N;
+    int rows;      // rows of L stored in `buf` (K, or K + n when right-hand sides rode along)
+};
+
+// cp_create zero-initialises every field (new cp_handle_s()) and sets device and num_sms.
 struct cp_handle_s {
     int device;
     int num_sms;
-    void *ws;          // scratch, grown on demand
-    size_t ws_bytes;
+    cp_buffer ws;      // scratch
     void *tmap_encode; // cuTensorMapEncodeTiled entry point (resolved lazily)
     // look-ahead of the blocked Cholesky (ls.cu): low-priority side stream + fork/join events, created lazily
     cudaStream_t side;   // urgent look-ahead: the updates the chain will need within the next few panels
     cudaStream_t bulk;   // the rest of every pair's trailing update (long kernels with slack): never ahead of `side` work
     cudaEvent_t ev_panel, ev_side, ev_bulk;
-    bool potrf_configured;  // opt-in shared memory of potrf128 set on this handle's device
-    // factor kept between cp_ls_factor and cp_ls_resolve (own allocation: the scratch above is reused by every call)
-    void *fac;
-    size_t fac_bytes;
-    int fac_K, fac_Kfull;
-    int64_t fac_N;
-    int fac_rows;  // rows of L stored in `fac` (Ksel, or Ksel + n when right-hand sides rode along)
+    cp_kept_factor fac;
     // second scratch: temporaries of an entry point that calls another one (cp_ls_residual -> cp_gram), which
     // carves its own scratch out of `ws`
-    void *aux;
-    size_t aux_bytes;
+    cp_buffer aux;
     // cp_gram_profile: CUDA events around the tensor-core GEMM kernel of cp_gram (bench.py's roofline of that kernel)
     bool gram_profile;
     cudaEvent_t ev_gram0, ev_gram1;
     // tensor-core (split-precision) bulk products of the least-squares solver (gemm_tc.cu): on/off per handle
     // (cp_ls_tensor_cores) and one operand buffer per stream the solver issues work on (caller's, side, bulk)
     bool ls_tc;
-    void *tcbuf[3];
-    size_t tcbuf_bytes[3];
+    cp_buffer tcbuf[3];
 };
 
 // Entry points run on the handle's device whatever the caller's current device is (restored on return).

@@ -211,19 +211,9 @@ int cp_gemm_tc_f64(cp_handle_t h, int slot, const double *A, int64_t lda, const 
     const int rowsA = cp_cdiv(M, TILE) * TILE, rowsB = same ? rowsA : cp_cdiv(Nn, TILE) * TILE;
     const size_t needA = 2 * (size_t)rowsA * Rp * sizeof(__half), needB = same ? 0 : 2 * (size_t)rowsB * Rp * sizeof(__half);
     const size_t need = cp_align_up(needA, 256) + cp_align_up(needB, 256) + cp_align_up((size_t)(rowsA + 2 * rowsB) * 8, 256);
-    if (need > h->tcbuf_bytes[slot]) {
-        if (h->tcbuf[slot]) CP_CUDA(cudaFree(h->tcbuf[slot]));  // synchronises: nothing in flight uses the old block
-        h->tcbuf[slot] = nullptr;
-        h->tcbuf_bytes[slot] = 0;
-        const size_t want = cp_align_up(need + need / 4, (size_t)1 << 20);
-        cudaError_t e = cudaMalloc(&h->tcbuf[slot], want);
-        if (e != cudaSuccess) {
-            cudaGetLastError();
-            CP_FAIL(CP_ERR_WORKSPACE, "tensor-core GEMM operand buffer of %zu bytes failed: %s", want, cudaGetErrorString(e));
-        }
-        h->tcbuf_bytes[slot] = want;
-    }
-    cp_carver cv(h->tcbuf[slot]);
+    int rc = cp_buffer_reserve(h->tcbuf[slot], need, 4, "tensor-core GEMM operand buffer");
+    if (rc) return rc;
+    cp_carver cv(h->tcbuf[slot].ptr);
     __half *opA = cv.take<__half>(2 * (size_t)rowsA * Rp);
     __half *opB = same ? opA : cv.take<__half>(2 * (size_t)rowsB * Rp);
     double *invA = cv.take<double>(rowsA + 2 * rowsB);
@@ -242,7 +232,7 @@ int cp_gemm_tc_f64(cp_handle_t h, int slot, const double *A, int64_t lda, const 
         CP_CHECK_LAUNCH();
     }
     CUtensorMap mapA, mapB;
-    int rc = make_map16(h, &mapA, opA, Rp, 2 * (int64_t)rowsA, TILE);
+    rc = make_map16(h, &mapA, opA, Rp, 2 * (int64_t)rowsA, TILE);
     if (rc) return rc;
     rc = make_map16(h, &mapB, opB, Rp, 2 * (int64_t)rowsB, TILE);
     if (rc) return rc;

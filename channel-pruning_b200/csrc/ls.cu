@@ -43,6 +43,12 @@ constexpr size_t P128_SMEM =
     (size_t)(PB * LDA_S + 2 * NSB * SB * LDX_S + 3 * SB * LDX_S + 3 * PB + 2 * SB) * sizeof(double);
 
 // ---------------------------------------------------------------- assemble
+// centred right-hand side t at column sj:  Bxy[sj, t] - sx_sj sy_t / N
+__device__ __forceinline__ double centred_rhs(const double *__restrict__ Bxy, const double *__restrict__ sx,
+                                              const double *__restrict__ sy, double invN, int n, int sj, int t) {
+    return Bxy[(int64_t)sj * n + t] - sx[sj] * sy[t] * invN;
+}
+
 // M rows 0..Ks-1    : G[sel_i, sel_j] - sx_i sx_j / N   (lower triangle only)
 // M rows Ks..Ks+n-1 : Bxy[sel_j, t]   - sx_j sy_t / N   (right-hand sides, transposed)
 __global__ void __launch_bounds__(256)
@@ -60,8 +66,7 @@ ls_assemble(const double *__restrict__ G, const double *__restrict__ Bxy, const 
         M[(int64_t)i * ld + j] = v;
         if (i == j) diag0[i] = v;
     } else if (Bxy) {
-        const int t = i - Ks;
-        M[(int64_t)i * ld + j] = Bxy[(int64_t)sj * n + t] - sx[sj] * sy[t] * invN;
+        M[(int64_t)i * ld + j] = centred_rhs(Bxy, sx, sy, invN, n, sj, i - Ks);
     }
 }
 
@@ -150,10 +155,24 @@ struct MmTask {
     int nterm;
     MmTerm t[3];
 };
-// Block products on the FP64 tensor path: four warps per task, one 16 x 16 quadrant each (2 x 2 m8n8k4 tiles), so the
-// twelve warps of a three-task phase sit on all four schedulers (rather than a 2 x 4 register micro-tile per thread on
-// 128 threads per task).
-// Fragment loads: A[r][q], B[c][q] with q contiguous (the MmTerm convention).
+// acc += one warp's 16 x 16 block of A B' over 32 reduction elements, as 2 x 2 m8n8k4 tiles (acc[u][v]: A rows
+// 8u to 8u+7, B rows 8v to 8v+7).  pa, pb: the lane's first fragment elements (row lane / 4, element lane % 4); sa8,
+// sb8: the distance of eight rows of A and of B.  Fragment loads: A[r][q], B[c][q] with q contiguous.
+__device__ __forceinline__ void dmma_block16(double (&acc)[2][2][2], const double *pa, int sa8, const double *pb,
+                                             int sb8) {
+#pragma unroll
+    for (int q = 0; q < SB; q += 4) {
+        const double a0 = pa[q], a1 = pa[sa8 + q], b0 = pb[q], b1 = pb[sb8 + q];
+        cpgemm::dmma884(acc[0][0][0], acc[0][0][1], a0, b0);
+        cpgemm::dmma884(acc[0][1][0], acc[0][1][1], a0, b1);
+        cpgemm::dmma884(acc[1][0][0], acc[1][0][1], a1, b0);
+        cpgemm::dmma884(acc[1][1][0], acc[1][1][1], a1, b1);
+    }
+}
+
+// Block products on the FP64 tensor path: four warps per task, one 16 x 16 quadrant each, so the twelve warps of a
+// three-task phase sit on all four schedulers (rather than a 2 x 4 register micro-tile per thread on 128 threads per
+// task).
 __device__ __forceinline__ void run_tasks_mma(const MmTask *tasks, int ntask) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (warp >= ntask * 4) return;
@@ -165,23 +184,9 @@ __device__ __forceinline__ void run_tasks_mma(const MmTask *tasks, int ntask) {
     for (int u = 0; u < 2; ++u)
 #pragma unroll
         for (int v = 0; v < 2; ++v) acc[u][v][0] = acc[u][v][1] = 0.0;
-    for (int w = 0; w < tk.nterm; ++w) {
-        const double *ap = tk.t[w].A + (r0 + fr) * tk.t[w].sa + fk;
-        const double *bp = tk.t[w].B + (c0 + fr) * tk.t[w].sb + fk;
-        const int sa8 = 8 * tk.t[w].sa, sb8 = 8 * tk.t[w].sb;
-#pragma unroll
-        for (int q = 0; q < SB; q += 4) {
-            const double a0 = ap[q], a1 = ap[sa8 + q], b0 = bp[q], b1 = bp[sb8 + q];
-            asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
-                         : "+d"(acc[0][0][0]), "+d"(acc[0][0][1]) : "d"(a0), "d"(b0));
-            asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
-                         : "+d"(acc[0][1][0]), "+d"(acc[0][1][1]) : "d"(a0), "d"(b1));
-            asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
-                         : "+d"(acc[1][0][0]), "+d"(acc[1][0][1]) : "d"(a1), "d"(b0));
-            asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
-                         : "+d"(acc[1][1][0]), "+d"(acc[1][1][1]) : "d"(a1), "d"(b1));
-        }
-    }
+    for (int w = 0; w < tk.nterm; ++w)
+        dmma_block16(acc, tk.t[w].A + (r0 + fr) * tk.t[w].sa + fk, 8 * tk.t[w].sa,
+                     tk.t[w].B + (c0 + fr) * tk.t[w].sb + fk, 8 * tk.t[w].sb);
 #pragma unroll
     for (int u = 0; u < 2; ++u)
 #pragma unroll
@@ -286,25 +291,13 @@ potrf128(const double *__restrict__ A, int64_t lda, int nb, double *__restrict__
                 int bj = 0, l = blk;
                 while (l >= nb16 - bj) { l -= nb16 - bj; ++bj; }
                 const int bi = bj + l;
-                const double *pa = As + (r0 + 16 * bi + fr) * LDA_S + k0 + fk;
-                const double *pb = As + (r0 + 16 * bj + fr) * LDA_S + k0 + fk;
                 double acc[2][2][2];
 #pragma unroll
                 for (int u = 0; u < 2; ++u)
 #pragma unroll
                     for (int v = 0; v < 2; ++v) acc[u][v][0] = acc[u][v][1] = 0.0;
-#pragma unroll
-                for (int q = 0; q < SB; q += 4) {
-                    const double a0 = pa[q], a1 = pa[8 * LDA_S + q], b0 = pb[q], b1 = pb[8 * LDA_S + q];
-                    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
-                                 : "+d"(acc[0][0][0]), "+d"(acc[0][0][1]) : "d"(a0), "d"(b0));
-                    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
-                                 : "+d"(acc[0][1][0]), "+d"(acc[0][1][1]) : "d"(a0), "d"(b1));
-                    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
-                                 : "+d"(acc[1][0][0]), "+d"(acc[1][0][1]) : "d"(a1), "d"(b0));
-                    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
-                                 : "+d"(acc[1][1][0]), "+d"(acc[1][1][1]) : "d"(a1), "d"(b1));
-                }
+                dmma_block16(acc, As + (r0 + 16 * bi + fr) * LDA_S + k0 + fk, 8 * LDA_S,
+                             As + (r0 + 16 * bj + fr) * LDA_S + k0 + fk, 8 * LDA_S);
 #pragma unroll
                 for (int u = 0; u < 2; ++u)
 #pragma unroll
@@ -485,14 +478,6 @@ int ensure_side(cp_handle_t h, cudaStream_t stream) {
     return CP_OK;
 }
 
-int configure_potrf(cp_handle_t h) {
-    if (!h->potrf_configured) {  // the attribute is per device: remembered per handle (one handle = one device)
-        CP_CUDA(cudaFuncSetAttribute(potrf128, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P128_SMEM));
-        h->potrf_configured = true;
-    }
-    return CP_OK;
-}
-
 }  // namespace
 
 static inline int ngroups(int Kd) { return (Kd + GB - 1) / GB; }
@@ -520,14 +505,21 @@ static int merge_inverse(cp_handle_t h, double *X, const double *L21, int64_t ld
 // that end up holding the INVERSES of the 512-wide diagonal blocks of L (the 128-wide ones come out of potrf128; they
 // are merged pairwise, X21 = -X22 L21 X11, on the side stream while the factorisation proceeds); Tm: scratch of the
 // same size.  The substitutions then take ceil(Kd/512) steps instead of ceil(Kd/128).
+// Status: info receives the first failed pivot (1-based, 0: none), ratio the smallest pivot / original diagonal ratio,
+// copied to stat_out (when not NULL) once the factorisation is complete.
 static int chol_factor(cp_handle_t h, double *M, double *L, int64_t ld, int Kd, int nrhs, double *Xinv, double *Tm,
-                       const double *diag0, int32_t *info, double *ratio, cudaStream_t stream) {
+                       const double *diag0, int32_t *info, double *ratio, double *stat_out, cudaStream_t stream) {
     using namespace cpgemm;
     const int Ktot = Kd + nrhs;
     int rc = ensure_side(h, stream);
     if (rc) return rc;
-    rc = configure_potrf(h);
-    if (rc) return rc;
+    static cp_per_device_flag potrf_configured;
+    if (bool *done = potrf_configured.slot(); !*done) {
+        CP_CUDA(cudaFuncSetAttribute(potrf128, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P128_SMEM));
+        *done = true;
+    }
+    CP_CUDA(cudaMemsetAsync(info, 0, sizeof(int32_t), stream));
+    CP_CUDA(cudaMemsetAsync(ratio, 0x7f, sizeof(double), stream));  // 1.4e306: "no pivot seen yet"
     CP_CUDA(cudaMemsetAsync(Xinv, 0, xinv_elems(Kd) * sizeof(double), stream));
     // Trailing updates.  Panels are paired (e, o = e + 1).  What the chain needs next stays small and immediate:
     //   crit(p)   : block column p+1, inner dimension 128, on the caller's stream, 64 x 64 tiles
@@ -644,7 +636,20 @@ static int chol_factor(cp_handle_t h, double *M, double *L, int64_t ld, int Kd, 
     CP_CUDA(cudaStreamWaitEvent(stream, h->ev_side, 0));
     CP_CUDA(cudaEventRecord(h->ev_bulk, h->bulk));
     CP_CUDA(cudaStreamWaitEvent(stream, h->ev_bulk, 0));
+    if (stat_out) CP_CUDA(cudaMemcpyAsync(stat_out, ratio, sizeof(double), cudaMemcpyDeviceToDevice, stream));
     return CP_OK;
+}
+
+// The bulk update of a substitution step, C (n x Nn) -= A (n x R) b' (b as in dgemm).  tc: it may take the tensor cores.
+// Few right-hand sides: 128 x 128 tiles would leave most SMs idle on a 512-deep product, 64 x 64 tiles fill them.
+// Tensor-core mode: split-precision tiles (n >= 256 right-hand sides, a few column tiles) beat the fp64 pipe.
+template <bool B_NC>
+static int subst_update(cp_handle_t h, bool tc, const double *A, int64_t lda, const double *B, int64_t ldb, double *C,
+                        int64_t ldc, int n, int Nn, int R, cudaStream_t stream) {
+    using namespace cpgemm;
+    const bool use_tc = tc && h->ls_tc && n >= 256 && Nn >= 512;
+    const int tile = use_tc || num_tiles(n, Nn, TILES_ALL, BM) >= 2 * h->num_sms ? 128 : 64;
+    return dgemm<B_NC>(h, use_tc, tile, TILES_ALL, 0, A, lda, B, ldb, C, ldc, n, Nn, R, -1.0, 1.0, stream);
 }
 
 // Forward substitution of further right-hand sides: Zt (n x Kd, ld) is destroyed, F (n x Kd, ld) receives (L^-1 Rhs)'.
@@ -659,12 +664,8 @@ static int chol_forward(cp_handle_t h, const double *L, int64_t ld, int Kd, cons
         int rc = dgemm<false>(h, false, 64, TILES_ALL, 0, Zt + g0, ldz, Xg, GB, F + g0, ldz, n, gs, gs, 1.0, 0.0, stream);
         if (rc) return rc;
         if (Kd - g1 > 0) {  // Zt[:, g1:] -= F_g * L[g1:, g0:g1]'
-            // few right-hand sides: 128 x 128 tiles would leave most SMs idle on a 512-deep product, 64 x 64 tiles fill them
-            // tensor-core mode: split-precision tiles (n >= 256 right-hand sides, a few column tiles) beat the fp64 pipe
-            const bool use_tc = h->ls_tc && n >= 256 && Kd - g1 >= 512;
-            const int tile = use_tc || num_tiles(n, Kd - g1, TILES_ALL, BM) >= 2 * h->num_sms ? 128 : 64;
-            rc = dgemm<false>(h, use_tc, tile, TILES_ALL, 0, F + g0, ldz, L + (int64_t)g1 * ld + g0, ld, Zt + g1, ldz, n,
-                              Kd - g1, gs, -1.0, 1.0, stream);
+            rc = subst_update<false>(h, true, F + g0, ldz, L + (int64_t)g1 * ld + g0, ld, Zt + g1, ldz, n, Kd - g1, gs,
+                                     stream);
             if (rc) return rc;
         }
     }
@@ -684,10 +685,7 @@ static int chol_backward(cp_handle_t h, bool tc, const double *L, int64_t ld, in
         int rc = dgemm<true>(h, false, 64, TILES_ALL, 0, F + g0, ldf, Xg, GB, Wt + g0, ldw, n, gs, gs, 1.0, 0.0, stream);
         if (rc) return rc;
         if (g0 > 0) {  // F[:, 0:g0] -= Wt_g * L[g0:g0+gs, 0:g0]
-            const bool use_tc = tc && h->ls_tc && n >= 256 && g0 >= 512;
-            const int tile = use_tc || num_tiles(n, g0, TILES_ALL, BM) >= 2 * h->num_sms ? 128 : 64;
-            rc = dgemm<true>(h, use_tc, tile, TILES_ALL, 0, Wt + g0, ldw, L + (int64_t)g0 * ld, ld, F, ldf, n, g0, gs, -1.0,
-                             1.0, stream);
+            rc = subst_update<true>(h, tc, Wt + g0, ldw, L + (int64_t)g0 * ld, ld, F, ldf, n, g0, gs, stream);
             if (rc) return rc;
         }
     }
@@ -696,31 +694,54 @@ static int chol_backward(cp_handle_t h, bool tc, const double *L, int64_t ld, in
 
 static inline int64_t ld_for(int K) { return (K + 7) / 8 * 8; }
 
-// The factor (L: rows x ld, then the inverted 128 x 128 diagonal blocks, then the pivot-ratio scalar) lives in the
-// handle's own allocation, not in the shared scratch: it must survive the calls that follow a solve (refinement
-// against the same factor, cp_ls_resolve) and every other entry point reuses the scratch.
-static int fac_reserve(cp_handle_t h, size_t rows, int64_t ld, int Kd, double **L, double **Linv, double **Tm,
-                       double **ratio) {
-    const size_t need = cp_carver::need(rows * (size_t)ld, 8) + 2 * cp_carver::need(xinv_elems(Kd), 8) +
-                        cp_carver::need(1, 8);
-    if (need > h->fac_bytes) {
-        if (h->fac) CP_CUDA(cudaFree(h->fac));  // synchronises: nothing in flight still reads the old block
-        h->fac = nullptr;
-        h->fac_bytes = 0;
-        const size_t want = cp_align_up(need + need / 8, (size_t)1 << 20);
-        cudaError_t e = cudaMalloc(&h->fac, want);
-        if (e != cudaSuccess) {
-            cudaGetLastError();
-            CP_FAIL(CP_ERR_WORKSPACE, "factor allocation of %zu bytes failed: %s", want, cudaGetErrorString(e));
-        }
-        h->fac_bytes = want;
-    }
-    h->fac_K = 0;
-    cp_carver fc(h->fac);
-    *L = fc.take<double>(rows * (size_t)ld);
-    *Linv = fc.take<double>(xinv_elems(Kd));
-    *Tm = fc.take<double>(xinv_elems(Kd));
-    *ratio = fc.take<double>(1);
+// The kept factor (h->fac) lives in the handle's own allocation, not in the shared scratch: it must survive the calls
+// that follow a solve (refinement against the same factor, cp_ls_resolve), and every other entry point reuses the
+// scratch.  Layout: L (rows x ld_for(Kd)), the inverted 512-wide diagonal blocks, their scratch, the pivot ratio.
+struct FacParts {
+    double *L, *Linv, *Tm, *ratio;
+};
+static size_t fac_bytes(size_t rows, int Kd) {
+    return cp_carver::need(rows * ld_for(Kd), 8) + 2 * cp_carver::need(xinv_elems(Kd), 8) + cp_carver::need(1, 8);
+}
+static FacParts fac_carve(void *base, size_t rows, int Kd) {
+    cp_carver fc(base);
+    FacParts p;
+    p.L = fc.take<double>(rows * ld_for(Kd));
+    p.Linv = fc.take<double>(xinv_elems(Kd));
+    p.Tm = fc.take<double>(xinv_elems(Kd));
+    p.ratio = fc.take<double>(1);
+    return p;
+}
+
+// Assembles the centred Gram of the selected columns, with the n right-hand sides of Bxy as rows under it when Bxy is
+// given, factors it into the kept factor and records that on the handle, for cp_ls_resolve or the rest of
+// cp_ls_solve.  A call that fails leaves the handle without a factor.  Wt: n x ld_for(Ksel) of scratch for the caller.
+static int factor_and_keep(cp_handle_t h, const double *G, const double *Bxy, const double *sx, const double *sy,
+                           int64_t N, int K, int n, const int32_t *sel_cols, int Ksel, int32_t *info_out,
+                           double *stat_out, cudaStream_t stream, FacParts *fac, double **Wt) {
+    h->fac.K = 0;
+    const int64_t ld = ld_for(Ksel);
+    const size_t rows = (size_t)(Ksel + n);
+    int rc = cp_buffer_reserve(h->fac.buf, fac_bytes(rows, Ksel), 8, "factor allocation");
+    if (rc) return rc;
+    *fac = fac_carve(h->fac.buf.ptr, rows, Ksel);
+    void *ws = nullptr;
+    rc = cp_ws_reserve(h, cp_carver::need(rows * ld, 8) + cp_carver::need((size_t)n * ld, 8) + cp_carver::need(Ksel, 8),
+                       &ws);
+    if (rc) return rc;
+    cp_carver cv(ws);
+    double *M = cv.take<double>(rows * ld);
+    *Wt = cv.take<double>((size_t)n * ld);
+    double *diag0 = cv.take<double>(Ksel);
+    ls_assemble<<<dim3(cp_cdiv(Ksel, 256), Ksel + n), 256, 0, stream>>>(G, Bxy, sx, sy, 1.0 / (double)N, K, n, sel_cols,
+                                                                       Ksel, M, ld, diag0);
+    CP_CHECK_LAUNCH();
+    rc = chol_factor(h, M, fac->L, ld, Ksel, n, fac->Linv, fac->Tm, diag0, info_out, fac->ratio, stat_out, stream);
+    if (rc) return rc;
+    h->fac.K = Ksel;
+    h->fac.Kfull = K;
+    h->fac.N = N;
+    h->fac.rows = Ksel + n;
     return CP_OK;
 }
 
@@ -734,36 +755,15 @@ extern "C" int cp_ls_solve(cp_handle_t h, const double *G, const double *Bxy, co
                (long long)(N - 1), Ksel);
     CP_DEVICE_GUARD(h);
     cudaStream_t stream = (cudaStream_t)stream_;
+    FacParts f;
+    double *Wt = nullptr;
+    int rc = factor_and_keep(h, G, Bxy, sx, sy, N, K, n, sel_cols, Ksel, info_out, stat_out, stream, &f, &Wt);
+    if (rc) return rc;
     const int64_t ld = ld_for(Ksel);
-    const size_t nM = (size_t)(Ksel + n) * ld;
-    double *L = nullptr, *Linv = nullptr, *Tm = nullptr, *ratio = nullptr;
-    int rc = fac_reserve(h, (size_t)(Ksel + n), ld, Ksel, &L, &Linv, &Tm, &ratio);
+    rc = chol_backward(h, true, f.L, ld, Ksel, f.Linv, f.L + (int64_t)Ksel * ld, ld, Wt, ld, n, stream);
     if (rc) return rc;
-    const size_t need = cp_carver::need(nM, 8) + cp_carver::need((size_t)n * ld, 8) + cp_carver::need(Ksel, 8);
-    void *ws = nullptr;
-    rc = cp_ws_reserve(h, need, &ws);
-    if (rc) return rc;
-    cp_carver cv(ws);
-    double *M = cv.take<double>(nM);
-    double *Wt = cv.take<double>((size_t)n * ld);
-    double *diag0 = cv.take<double>(Ksel);
-    CP_CUDA(cudaMemsetAsync(info_out, 0, sizeof(int32_t), stream));
-    CP_CUDA(cudaMemsetAsync(ratio, 0x7f, sizeof(double), stream));  // 1.4e306: "no pivot seen yet"
-    const double invN = 1.0 / (double)N;
-    dim3 grid(cp_cdiv(Ksel, 256), Ksel + n);
-    ls_assemble<<<grid, 256, 0, stream>>>(G, Bxy, sx, sy, invN, K, n, sel_cols, Ksel, M, ld, diag0);
+    ls_output<<<n, 256, 0, stream>>>(Wt, ld, sx, sy, sel_cols, Ksel, 1.0 / (double)N, W_out, b_out, 0);
     CP_CHECK_LAUNCH();
-    rc = chol_factor(h, M, L, ld, Ksel, n, Linv, Tm, diag0, info_out, ratio, stream);
-    if (rc) return rc;
-    rc = chol_backward(h, true, L, ld, Ksel, Linv, L + (int64_t)Ksel * ld, ld, Wt, ld, n, stream);
-    if (rc) return rc;
-    ls_output<<<n, 256, 0, stream>>>(Wt, ld, sx, sy, sel_cols, Ksel, invN, W_out, b_out, 0);
-    CP_CHECK_LAUNCH();
-    if (stat_out) CP_CUDA(cudaMemcpyAsync(stat_out, ratio, sizeof(double), cudaMemcpyDeviceToDevice, stream));
-    h->fac_K = Ksel;  // the factor stays valid for cp_ls_resolve (refinement of this very solve)
-    h->fac_Kfull = K;
-    h->fac_N = N;
-    h->fac_rows = Ksel + n;
     return CP_OK;
 }
 
@@ -776,31 +776,10 @@ extern "C" int cp_ls_factor(cp_handle_t h, const double *G, const double *sx, in
     CP_REQUIRE(sel_cols || Ksel == K, "cp_ls_factor: sel_cols may be NULL only when every column is used");
     CP_REQUIRE(N - 1 >= Ksel, "cp_ls_factor: N-1=%lld < K'=%d: centred Gram is singular", (long long)(N - 1), Ksel);
     CP_DEVICE_GUARD(h);
-    cudaStream_t stream = (cudaStream_t)stream_;
-    const int64_t ld = ld_for(Ksel);
-    const size_t nM = (size_t)Ksel * ld;
-    double *L = nullptr, *Linv = nullptr, *Tm = nullptr, *ratio = nullptr;
-    int rc = fac_reserve(h, (size_t)Ksel, ld, Ksel, &L, &Linv, &Tm, &ratio);
-    if (rc) return rc;
-    void *ws = nullptr;
-    rc = cp_ws_reserve(h, cp_carver::need(nM, 8) + cp_carver::need(Ksel, 8), &ws);
-    if (rc) return rc;
-    cp_carver cv(ws);
-    double *M = cv.take<double>(nM);
-    double *diag0 = cv.take<double>(Ksel);
-    CP_CUDA(cudaMemsetAsync(info_out, 0, sizeof(int32_t), stream));
-    CP_CUDA(cudaMemsetAsync(ratio, 0x7f, sizeof(double), stream));  // 1.4e306: "no pivot seen yet"
-    dim3 grid(cp_cdiv(Ksel, 256), Ksel);
-    ls_assemble<<<grid, 256, 0, stream>>>(G, nullptr, sx, nullptr, 1.0 / (double)N, K, 0, sel_cols, Ksel, M, ld, diag0);
-    CP_CHECK_LAUNCH();
-    rc = chol_factor(h, M, L, ld, Ksel, 0, Linv, Tm, diag0, info_out, ratio, stream);
-    if (rc) return rc;
-    if (stat_out) CP_CUDA(cudaMemcpyAsync(stat_out, ratio, sizeof(double), cudaMemcpyDeviceToDevice, stream));
-    h->fac_K = Ksel;
-    h->fac_Kfull = K;
-    h->fac_N = N;
-    h->fac_rows = Ksel;
-    return CP_OK;
+    FacParts f;
+    double *Wt = nullptr;
+    return factor_and_keep(h, G, nullptr, sx, nullptr, N, K, 0, sel_cols, Ksel, info_out, stat_out,
+                           (cudaStream_t)stream_, &f, &Wt);
 }
 
 namespace {
@@ -811,8 +790,7 @@ rhs_assemble(const double *__restrict__ Bxy, const double *__restrict__ sx, cons
     const int j = blockIdx.x * 256 + threadIdx.x;
     const int t = blockIdx.y;
     if (j >= Ks) return;
-    const int sj = sel ? sel[j] : j;
-    Zt[(int64_t)t * ld + j] = Bxy[(int64_t)sj * n + t] - sx[sj] * sy[t] * invN;
+    Zt[(int64_t)t * ld + j] = centred_rhs(Bxy, sx, sy, invN, n, sel ? sel[j] : j, t);
 }
 }  // namespace
 
@@ -820,16 +798,14 @@ extern "C" int cp_ls_resolve(cp_handle_t h, const double *Bxy, const double *sx,
                              const int32_t *sel_cols, double *W_out, double *b_out, int accumulate,
                              cp_stream_t stream_) {
     CP_REQUIRE(h && Bxy && sx && sy && W_out && b_out, "cp_ls_resolve: NULL argument");
-    CP_REQUIRE(h->fac_K > 0, "cp_ls_resolve: no factor on this handle (call cp_ls_factor first)");
+    CP_REQUIRE(h->fac.K > 0, "cp_ls_resolve: no factor on this handle (call cp_ls_factor first)");
     CP_REQUIRE(n > 0, "cp_ls_resolve: bad shape");
-    CP_REQUIRE(sel_cols || h->fac_K == h->fac_Kfull, "cp_ls_resolve: sel_cols needed (the factor used a column subset)");
+    CP_REQUIRE(sel_cols || h->fac.K == h->fac.Kfull, "cp_ls_resolve: sel_cols needed (the factor used a column subset)");
     CP_DEVICE_GUARD(h);
     cudaStream_t stream = (cudaStream_t)stream_;
-    const int Ksel = h->fac_K;
+    const int Ksel = h->fac.K;
     const int64_t ld = ld_for(Ksel);
-    cp_carver fc(h->fac);
-    const double *L = fc.take<double>((size_t)h->fac_rows * ld);
-    const double *Linv = fc.take<double>(xinv_elems(Ksel));
+    const FacParts f = fac_carve(h->fac.buf.ptr, h->fac.rows, Ksel);
     void *ws = nullptr;
     int rc = cp_ws_reserve(h, 3 * cp_carver::need((size_t)n * ld, 8), &ws);
     if (rc) return rc;
@@ -837,12 +813,12 @@ extern "C" int cp_ls_resolve(cp_handle_t h, const double *Bxy, const double *sx,
     double *Zt = cv.take<double>((size_t)n * ld);
     double *F = cv.take<double>((size_t)n * ld);
     double *Wt = cv.take<double>((size_t)n * ld);
-    const double invN = 1.0 / (double)h->fac_N;
+    const double invN = 1.0 / (double)h->fac.N;
     rhs_assemble<<<dim3(cp_cdiv(Ksel, 256), n), 256, 0, stream>>>(Bxy, sx, sy, invN, n, sel_cols, Ksel, Zt, ld);
     CP_CHECK_LAUNCH();
-    rc = chol_forward(h, L, ld, Ksel, Linv, Zt, F, ld, n, stream);
+    rc = chol_forward(h, f.L, ld, Ksel, f.Linv, Zt, F, ld, n, stream);
     if (rc) return rc;
-    rc = chol_backward(h, true, L, ld, Ksel, Linv, F, ld, Wt, ld, n, stream);
+    rc = chol_backward(h, true, f.L, ld, Ksel, f.Linv, F, ld, Wt, ld, n, stream);
     if (rc) return rc;
     ls_output<<<n, 256, 0, stream>>>(Wt, ld, sx, sy, sel_cols, Ksel, invN, W_out, b_out, accumulate);
     CP_CHECK_LAUNCH();
@@ -1041,26 +1017,6 @@ __global__ void add_const_lower(double *__restrict__ M, int64_t ld, int N, doubl
     }
 }
 
-__global__ void __launch_bounds__(256)
-dual_output(const double *__restrict__ Wt, int64_t ld, const double *__restrict__ xmean,
-            const double *__restrict__ ymean, int Ks, double *__restrict__ W_out, double *__restrict__ b_out) {
-    __shared__ double red[256];
-    const int t = blockIdx.x;
-    double s = 0.0;
-    for (int i = threadIdx.x; i < Ks; i += 256) {
-        const double w = Wt[(int64_t)t * ld + i];
-        W_out[(int64_t)t * Ks + i] = w;
-        s = fma(xmean[i], w, s);
-    }
-    red[threadIdx.x] = s;
-    __syncthreads();
-    for (int w = 128; w > 0; w >>= 1) {
-        if (threadIdx.x < w) red[threadIdx.x] += red[threadIdx.x + w];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) b_out[t] = ymean[t] - red[0];
-}
-
 }  // namespace
 
 extern "C" int cp_ls_solve_dual(cp_handle_t h, const float *X, int64_t N, int K, int64_t ldx, const void *Yraw,
@@ -1097,8 +1053,6 @@ extern "C" int cp_ls_solve_dual(cp_handle_t h, const float *X, int64_t N, int K,
     double *ymean = cv.take<double>(n);
     double *diag0 = cv.take<double>(Ni);
     double *ratio = cv.take<double>(1);
-    CP_CUDA(cudaMemsetAsync(info_out, 0, sizeof(int32_t), stream));
-    CP_CUDA(cudaMemsetAsync(ratio, 0x7f, sizeof(double), stream));  // 1.4e306: "no pivot seen yet"
     colmean_sel<float><<<cp_cdiv(Ksel, 32), 256, 0, stream>>>(X, ldx, sel_cols, Ksel, N, nullptr, xmean);
     CP_CHECK_LAUNCH();
     if (y_dtype == CP_F32)
@@ -1118,15 +1072,14 @@ extern "C" int cp_ls_solve_dual(cp_handle_t h, const float *X, int64_t N, int K,
     else
         dual_rhs<double><<<dim3(cp_cdiv(Ni, 256), n), 256, 0, stream>>>((const double *)Yraw, ldy, y_bias, ymean, N, n, M, ldm);
     CP_CHECK_LAUNCH();
-    rc = chol_factor(h, M, L, ldm, Ni, n, Linv, Tm, diag0, info_out, ratio, stream);
+    rc = chol_factor(h, M, L, ldm, Ni, n, Linv, Tm, diag0, info_out, ratio, stat_out, stream);
     if (rc) return rc;
     rc = chol_backward(h, false, L, ldm, Ni, Linv, L + (int64_t)Ni * ldm, ldm, At, ldm, n, stream);
     if (rc) return rc;
     // Wt = At * Xc   (C[t, i] = sum_r At[t, r] * Xc[r, i])
     rc = dgemm<true>(h, false, 128, TILES_ALL, 0, At, ldm, Xc, ldc, Wt, ldc, n, Ksel, Ni, 1.0, 0.0, stream);
     if (rc) return rc;
-    dual_output<<<n, 256, 0, stream>>>(Wt, ldc, xmean, ymean, Ksel, W_out, b_out);
+    ls_output<<<n, 256, 0, stream>>>(Wt, ldc, xmean, ymean, nullptr, Ksel, 1.0, W_out, b_out, 0);
     CP_CHECK_LAUNCH();
-    if (stat_out) CP_CUDA(cudaMemcpyAsync(stat_out, ratio, sizeof(double), cudaMemcpyDeviceToDevice, stream));
     return CP_OK;
 }

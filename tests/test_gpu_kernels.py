@@ -257,11 +257,23 @@ def test_ls_solve_matches_lstsq(engine, N, K, n, nsel):
     Y = (X @ r.standard_normal((K, n)) + r.standard_normal((N, n))).astype(np.float32)
     sel = np.sort(r.choice(K, nsel, replace=False)).astype(np.int32)
     g = engine.gram(_dev(X, engine), _dev(Y, engine), mode=0)
-    W, b, info, _ = engine.ls_solve(g, _dev(sel, engine))
+    sel_d = _dev(sel, engine)
+    W, b, info, _ = engine.ls_solve(g, sel_d)
     assert int(info.cpu()[0]) == 0
+    # the same system factored alone, then solved against the kept factor
+    info, _ = engine.ls_factor(g, sel_d)
+    assert int(info.cpu()[0]) == 0
+    Wr, br = engine.ls_resolve(g["B"], g["sx"], g["sy"], sel_d)
     coef, icpt = O.linear_regression(X[:, sel].astype(np.float64), Y.astype(np.float64))
-    assert np.linalg.norm(W.cpu().numpy() - coef) <= 1e-9 * np.linalg.norm(coef)
-    np.testing.assert_allclose(b.cpu().numpy(), icpt, atol=1e-9 * max(1, np.abs(icpt).max()))
+    for Wx, bx in ((W, b), (Wr, br)):
+        assert np.linalg.norm(Wx.cpu().numpy() - coef) <= 1e-9 * np.linalg.norm(coef)
+        np.testing.assert_allclose(bx.cpu().numpy(), icpt, atol=1e-9 * max(1, np.abs(icpt).max()))
+    # accumulate_into adds the solution to the given tensors in place
+    W1, b1 = Wr.cpu().numpy(), br.cpu().numpy()
+    Wa, ba = engine.ls_resolve(g["B"], g["sx"], g["sy"], sel_d, accumulate_into=(Wr, br))
+    assert Wa is Wr and ba is br
+    np.testing.assert_array_equal(Wr.cpu().numpy(), 2 * W1)
+    np.testing.assert_array_equal(br.cpu().numpy(), 2 * b1)
 
 
 def test_ls_solve_dual_minimum_norm(engine):
