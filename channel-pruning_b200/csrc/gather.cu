@@ -12,7 +12,8 @@
 // granularity -- that over-fetch is inherent to reading k-wide windows out of NCHW.
 // NHWC path: a window row is k*c contiguous floats; the CTA stages the k*k x c tile
 // in shared memory with coalesced loads (channel fastest) and writes it back
-// transposed to (c, k*k) column order, again coalesced.
+// transposed to (c, k*k) column order, again coalesced.  NHWC maps in HBM mostly take the TMA kernel (gather_tma.cu),
+// NHWC maps in pinned host memory the in-place reader of gather_host.cu.
 // Element type of the map: fp32, bf16 or fp16 (template parameter T, fmap_types.cuh).  X and Y are fp32 in every
 // case; the ReLU is applied to the widened value with the fp32 kernel's expression, so -0, inf and NaN come out as the
 // fp32 kernel gives them for the widened map.
@@ -122,6 +123,10 @@ bool cp_gather_tma_eligible(const void *fmap, int esize, int c, int k, float *X_
 int cp_patch_gather_tma(cp_handle_t h, const void *fmap, int fmap_dtype, int nbatch, int B, int c, int H, int W,
                         const int32_t *randx, const int32_t *randy, int P, int k, int pad, int stride, int relu,
                         float *X_out, int64_t ldx, cudaStream_t stream);
+// gather_host.cu
+int cp_patch_gather_nhwc_host(const void *fmap, int fmap_dtype, int nbatch, int B, int c, int H, int W,
+                              const int32_t *randx, const int32_t *randy, int P, int k, int pad, int stride, int relu,
+                              float *X_out, int64_t ldx, cudaStream_t stream);
 
 template <typename T>
 static void launch_patch_gather_simt(const T *fmap, int layout, bool host_src, int64_t rows,
@@ -172,6 +177,13 @@ extern "C" int cp_patch_gather_typed(cp_handle_t h, const void *fmap, int fmap_d
     } else {
         const size_t smem = (size_t)k * k * (NHWC_CT + 1) * sizeof(float);
         CP_REQUIRE(smem <= 48 * 1024, "cp_patch_gather: kernel_size %d too large for the NHWC tile", k);
+        // NHWC map in pinned host memory: whole window rows as 16-byte reads over PCIe (gather_host.cu)
+        cudaPointerAttributes pa;
+        const bool host_nhwc = cudaPointerGetAttributes(&pa, fmap) == cudaSuccess && pa.type == cudaMemoryTypeHost;
+        (void)cudaGetLastError();
+        if (host_nhwc)
+            return cp_patch_gather_nhwc_host(fmap, fmap_dtype, nbatch, B, c, H, W, randx, randy, P, k, pad, stride,
+                                             relu, X_out, ldx, stream);
     }
     if (fmap_dtype == CP_F32)
         launch_patch_gather_simt((const float *)fmap, layout, host_src, rows, B, c, H, W, randx, randy, P, k, pad,

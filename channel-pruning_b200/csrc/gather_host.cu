@@ -1,0 +1,180 @@
+// In-place reader of channels-last (NHWC) feature maps in pinned host memory: the patch gather of the host-resident
+// input path for maps a channels_last forward hands over (cp_patch_gather_typed, layout NHWC, map in page-locked host
+// memory mapped under UVA).
+//
+// Over PCIe a gather costs read requests, not bytes.  In NHWC the in-bounds taps of a window row are one contiguous
+// run of (taps x c) elements, so the reader fetches each run as 16-byte vectors, consecutive threads on consecutive
+// addresses: every 128-byte line of the run is requested once and nearly all of its bytes are used (NCHW: c*k runs of
+// k elements per window).
+// A work unit is one (output row, channel chunk).  Its k*k x ct sub-window is copied by cp.async into a shared-memory
+// stage; while one unit is widened, transposed to the (c, k*k) column order and stored, the copies of the next NS - 1
+// units of the CTA are in flight.  Chunks keep a stage within NHWC_HOST_SMEM / NS bytes whatever c and k (a c = 2048,
+// k = 3 fp32 window is 72 KB).  A small persistent grid strides over the units: the zero-copy gathers run beside other
+// layers' searches and Grams, which need the SMs.
+// Maps whose channel stride or base address is not a multiple of 16 bytes (c = 3, 5, 12 in fp32; odd c in 16 bit)
+// take plain element loads into the same stages: correct for every c, not tuned.
+// The output is bit for bit that of the HBM NHWC kernels: zero outside the map, cp_widen, then fmaxf for the ReLU.
+#include "common.cuh"
+#include "fmap_types.cuh"
+
+namespace {
+
+constexpr int NHWC_HOST_SMEM = 48 * 1024;  // shared memory of a CTA (all stages)
+constexpr int NHWC_HOST_PAD = 16;          // bytes after each tap of a stage: keeps 16-byte alignment, spreads banks
+
+struct NhwcHostGeom {
+    int B, P, c, H, W, k, pad, stride;
+    int ct;       // channels per chunk (the last chunk may be shorter)
+    int nchunk;   // chunks per window
+    int tap;      // bytes per tap in a stage: ct * esize + NHWC_HOST_PAD
+    int stage;    // bytes per stage
+    int vec;      // 16-byte copies (c * esize % 16 == 0, 16-byte aligned map)
+};
+
+__device__ __forceinline__ void nh_cp_async16(void *smem, const void *gmem) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem)),
+                 "l"(gmem) : "memory");
+}
+
+// Starts the copy of unit u into `stage`: 16-byte cp.async requests, or (vec == 0) plain element loads.
+template <typename T>
+__device__ __forceinline__ void nhwc_host_fetch(const T *__restrict__ fmap, const int32_t *__restrict__ randx,
+                                                const int32_t *__restrict__ randy, const NhwcHostGeom &g, int64_t u,
+                                                unsigned char *stage) {
+    const int64_t r = u / g.nchunk;
+    const int a0 = (int)(u - r * g.nchunk) * g.ct;
+    const int ct = min(g.ct, g.c - a0);
+    const int k2 = g.k * g.k;
+    const int64_t bp = r / g.B;
+    const int img = (int)(bp / g.P) * g.B + (int)(r % g.B);
+    const int y0 = g.stride * randx[bp] - g.pad;
+    const int x0 = g.stride * randy[bp] - g.pad;
+    const T *src = fmap + (int64_t)img * g.H * g.W * g.c + a0;
+    if (g.vec) {
+        constexpr int VE = 16 / sizeof(T);  // elements per copy
+        const int nv = ct / VE;
+        for (int e = threadIdx.x; e < k2 * nv; e += blockDim.x) {
+            const int p = e / nv, j = e - p * nv;
+            const int py = p / g.k, px = p - py * g.k;
+            const int yy = y0 + py, xx = x0 + px;
+            if (yy >= 0 && yy < g.H && xx >= 0 && xx < g.W)
+                nh_cp_async16(stage + p * g.tap + j * 16, src + ((int64_t)yy * g.W + xx) * g.c + j * VE);
+        }
+    } else {
+        for (int e = threadIdx.x; e < k2 * ct; e += blockDim.x) {
+            const int p = e / ct, a = e - p * ct;
+            const int py = p / g.k, px = p - py * g.k;
+            const int yy = y0 + py, xx = x0 + px;
+            if (yy >= 0 && yy < g.H && xx >= 0 && xx < g.W)
+                reinterpret_cast<T *>(stage + p * g.tap)[a] = __ldg(src + ((int64_t)yy * g.W + xx) * g.c + a);
+        }
+    }
+}
+
+// Writes unit u from its stage: column a*k*k + p of the chunk, zero for taps outside the map.
+template <typename T>
+__device__ __forceinline__ void nhwc_host_store(const int32_t *__restrict__ randx, const int32_t *__restrict__ randy,
+                                                float *__restrict__ X, int64_t ldx, const NhwcHostGeom &g, int64_t u,
+                                                const unsigned char *stage, int relu) {
+    const int64_t r = u / g.nchunk;
+    const int a0 = (int)(u - r * g.nchunk) * g.ct;
+    const int ct = min(g.ct, g.c - a0);
+    const int k2 = g.k * g.k;
+    const int64_t bp = r / g.B;
+    const int y0 = g.stride * randx[bp] - g.pad;
+    const int x0 = g.stride * randy[bp] - g.pad;
+    float *dst = X + r * ldx + (int64_t)a0 * k2;
+    for (int e = threadIdx.x; e < k2 * ct; e += blockDim.x) {
+        const int a = e / k2, p = e - a * k2;
+        const int py = p / g.k, px = p - py * g.k;
+        const int yy = y0 + py, xx = x0 + px;
+        float v = 0.f;
+        if (yy >= 0 && yy < g.H && xx >= 0 && xx < g.W) v = cp_widen(reinterpret_cast<const T *>(stage + p * g.tap)[a]);
+        if (relu) v = fmaxf(v, 0.f);
+        dst[e] = v;
+    }
+}
+
+// NS stages: unit u + i * gridDim.x is copied into stage (it + i) % NS while unit u is stored.
+template <int NS, typename T>
+__global__ void __launch_bounds__(256)
+patch_gather_nhwc_host(const T *__restrict__ fmap, const int32_t *__restrict__ randx,
+                       const int32_t *__restrict__ randy, float *__restrict__ X, int64_t ldx, int64_t units,
+                       NhwcHostGeom g, int relu) {
+    extern __shared__ __align__(16) unsigned char nh_smem[];
+    const int64_t step = gridDim.x;
+#pragma unroll
+    for (int i = 0; i < NS - 1; ++i) {
+        const int64_t ui = blockIdx.x + i * step;
+        if (ui < units) nhwc_host_fetch(fmap, randx, randy, g, ui, nh_smem + i * g.stage);
+        asm volatile("cp.async.commit_group;" ::: "memory");
+    }
+    int it = 0;
+    for (int64_t u = blockIdx.x; u < units; u += step, ++it) {
+        const int64_t un = u + (NS - 1) * step;
+        if (un < units) nhwc_host_fetch(fmap, randx, randy, g, un, nh_smem + ((it + NS - 1) % NS) * g.stage);
+        asm volatile("cp.async.commit_group;" ::: "memory");
+        asm volatile("cp.async.wait_group %0;" ::"n"(NS - 1) : "memory");  // unit u's copies have landed
+        __syncthreads();
+        nhwc_host_store<T>(randx, randy, X, ldx, g, u, nh_smem + (it % NS) * g.stage, relu);
+        __syncthreads();  // the stage is refilled NS - 1 units later
+    }
+    asm volatile("cp.async.wait_group 0;" ::: "memory");
+}
+
+}  // namespace
+
+// Geometry of the reader for one map: channel chunk and stage sizes for NS stages.  Returns false when one copy per
+// tap does not fit a stage (never for the k <= 9 that cp_patch_gather_typed lets through).
+static bool nhwc_host_geom(NhwcHostGeom &g, const void *fmap, int esize, int B, int P, int c, int H, int W, int k,
+                           int pad, int stride, int ns) {
+    const int k2 = k * k;
+    g.B = B, g.P = P, g.c = c, g.H = H, g.W = W, g.k = k, g.pad = pad, g.stride = stride;
+    g.vec = (c * esize) % 16 == 0 && ((uintptr_t)fmap & 15) == 0;
+    const int ve = g.vec ? 16 / esize : 1;
+    int ctmax = (NHWC_HOST_SMEM / ns / k2 - NHWC_HOST_PAD) / esize;
+    ctmax -= ctmax % ve;
+    if (ctmax < ve) return false;
+    g.nchunk = cp_cdiv(c, ctmax);
+    g.ct = cp_cdiv(cp_cdiv(c, g.nchunk), ve) * ve;  // balanced chunks, whole 16-byte copies
+    g.nchunk = cp_cdiv(c, g.ct);
+    g.tap = g.ct * esize + NHWC_HOST_PAD;
+    g.stage = k2 * g.tap;
+    return true;
+}
+
+template <int NS, typename T>
+static void launch_nhwc_host(const T *fmap, const NhwcHostGeom &g, int64_t rows, const int32_t *randx,
+                             const int32_t *randy, int relu, float *X_out, int64_t ldx, int ncta, cudaStream_t stream) {
+    const int64_t units = rows * g.nchunk;
+    const unsigned grid = (unsigned)(units < ncta ? units : ncta);
+    patch_gather_nhwc_host<NS, T><<<grid, 256, (size_t)NS * g.stage, stream>>>(fmap, randx, randy, X_out, ldx, units,
+                                                                                g, relu);
+}
+
+// Grid and pipeline depth of the reader (profiles/host_nhwc_ctas.cu; H100 80GB HBM3 SXM, 700 W; DESIGN.md section 3).
+// The link bounds it: conv3_2 / conv4_2 at N = 5000 read 23-27 GB/s of window bytes with 16 to 132 CTAs.  With two
+// stages 32 CTAs are within the spread of 64 and 132 in fp32 and bf16 and leave the other SMs to the layers that
+// search and factor meanwhile; with one stage (no copy in flight while a unit is stored) 16 CTAs lose 30 % in bf16.
+constexpr int CP_HOST_NHWC_GATHER_CTAS = 32;
+constexpr int CP_HOST_NHWC_STAGES = 2;
+
+int cp_patch_gather_nhwc_host(const void *fmap, int fmap_dtype, int nbatch, int B, int c, int H, int W,
+                              const int32_t *randx, const int32_t *randy, int P, int k, int pad, int stride, int relu,
+                              float *X_out, int64_t ldx, cudaStream_t stream) {
+    NhwcHostGeom g;
+    CP_REQUIRE(nhwc_host_geom(g, fmap, cp_fmap_esize(fmap_dtype), B, P, c, H, W, k, pad, stride, CP_HOST_NHWC_STAGES),
+               "cp_patch_gather: kernel_size %d too large for the NHWC host reader", k);
+    const int64_t rows = (int64_t)nbatch * P * B;
+    if (fmap_dtype == CP_F32)
+        launch_nhwc_host<CP_HOST_NHWC_STAGES>((const float *)fmap, g, rows, randx, randy, relu, X_out, ldx,
+                                              CP_HOST_NHWC_GATHER_CTAS, stream);
+    else if (fmap_dtype == CP_BF16)
+        launch_nhwc_host<CP_HOST_NHWC_STAGES>((const __nv_bfloat16 *)fmap, g, rows, randx, randy, relu, X_out, ldx,
+                                              CP_HOST_NHWC_GATHER_CTAS, stream);
+    else
+        launch_nhwc_host<CP_HOST_NHWC_STAGES>((const __half *)fmap, g, rows, randx, randy, relu, X_out, ldx,
+                                              CP_HOST_NHWC_GATHER_CTAS, stream);
+    CP_CHECK_LAUNCH();
+    return CP_OK;
+}

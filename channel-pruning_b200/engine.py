@@ -232,7 +232,7 @@ class Engine:
     # ------------------------------------------------------------------ kernels
     def patch_gather(self, fmap, randx, randy, B, P, k, pad, stride, relu=True, layout="nchw", out=None):
         """fmap: (nbatch*B, c, H, W) [nchw] or (nbatch*B, H, W, c) [nhwc], float32 / bfloat16 / float16, on device
-        or (nchw) in pinned host memory; randx/randy: (nbatch, P) int32 on device.  Returns X (nbatch*P*B, c*k*k)
+        or in pinned host memory (read in place over PCIe); randx/randy: (nbatch, P) int32 on device.  Returns X (nbatch*P*B, c*k*k)
         fp32 -- 16-bit maps are widened exactly, so X equals the X of fmap.float()."""
         dt = fmap_dtype_code(fmap.dtype)
         assert fmap.is_contiguous()

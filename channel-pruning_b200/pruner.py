@@ -105,7 +105,8 @@ class LayerResult:
 def prune_layers(eng: Engine, shapes, datas, right0=1e-3, rank_tol=.1, from_host=False, to_host=False, trace=None):
     """Runs the layer problems ``shapes[i]`` / ``datas[i]`` (see synth.make_problem_device) on
     ``eng``.  from_host: feature maps are taken from pinned host memory (datas[i]['fmap_host'], float32, bfloat16
-    or float16) and copied in the pipeline; to_host: results are copied back to pinned host memory.
+    or float16, laid out as datas[i]['host_layout']: 'nchw' (default) or 'nhwc') and copied in the pipeline; to_host:
+    results are copied back to pinned host memory.
     trace: optional dict; filled with {layer name: [(label, timing event), ...]} plus '_t0' (device timeline
     of the step: profiles/e2e_breakdown.py prints it).
     Batch mode: the problems are INDEPENDENT -- every alpha search starts from ``right0`` and the seeds come with the
@@ -133,19 +134,32 @@ def prune_layers(eng: Engine, shapes, datas, right0=1e-3, rank_tol=.1, from_host
 
 # read requests per second of the in-place gather over PCIe (profiles/zc_rate.py; H100 80GB HBM3 SXM, PCIe 5)
 ZC_LINES_PER_S = 2.6e8
+# full 128-byte lines per second of the in-place NHWC reader, whose requests are whole lines of contiguous window rows
+# (profiles/host_nhwc.py, conv2_2 to conv5_1 at N = 5000, fp32 and bf16: 6.8e7 to 7.7e7, median 7.1e7, about 9 GB/s,
+# on an H100 80GB HBM3 SXM at 700 W whose NCHW reader ran at 2.2e8 to 3.0e8 lines/s, the regime of ZC_LINES_PER_S;
+# another such card read 1.9e8 NHWC and 5.7e8 NCHW lines/s: the host link varies, the ratio of the two readers not)
+ZC_NHWC_LINES_PER_S = 7.1e7
 
 
-def zero_copy_lines(s, esize=4):
-    """128-byte lines the in-place gather touches in host memory (the k rows of a window are W*esize bytes apart;
-    esize: bytes per map element)."""
+def zero_copy_lines(s, esize=4, layout="nchw"):
+    """128-byte lines the in-place gather touches in host memory (esize: bytes per map element).
+    nchw: c*k runs of k elements per window; the k rows of a channel are W*esize bytes apart.
+    nhwc: k runs of k*c*esize contiguous bytes per window, plus one line per run when the pixel stride c*esize is
+    not a multiple of 128 bytes (a run may then start inside a line).  An upper bound for a map whose base is
+    128-byte aligned: clipping at the border only removes lines."""
+    if layout == "nhwc":
+        run = s.k * s.c * esize
+        per_run = -(-run // 128) + (1 if (s.c * esize) % 128 else 0)
+        return s.N * s.k * per_run
     row = s.W * esize if hasattr(s, "W") else esize * 64
     lines = min(s.k, -(-((s.k - 1) * row + s.k * esize) // 128) + 1) if s.k > 1 else 1
     return s.N * s.c * lines
 
 
-def _zero_copy_seconds(s, esize=4):
+def _zero_copy_seconds(s, esize=4, layout="nchw"):
     """Model of the in-place gather over PCIe: it is bound by the number of read requests."""
-    return zero_copy_lines(s, esize) / ZC_LINES_PER_S
+    rate = ZC_NHWC_LINES_PER_S if layout == "nhwc" else ZC_LINES_PER_S
+    return zero_copy_lines(s, esize, layout) / rate
 
 
 def _element_size(fmap):
@@ -159,7 +173,7 @@ def h2d_plan(shapes, datas, from_host):
     moves the whole map at full PCIe bandwidth, gather from HBM).  DMA pays off when the windows cover most of
     the map (small spatial maps: conv5_x).  CPB200_DMA_MAX_MB caps the size of a map that may be staged.
     The reader and the copy engine share the link, so moving a map from one to the other buys nothing unless it
-    removes bytes."""
+    removes bytes.  The reader's cost follows the host map's layout (datas[i]['host_layout'], 'nchw' by default)."""
     if from_host == "zc":
         return ["zc"] * len(shapes)
     if from_host == "copy":
@@ -171,7 +185,8 @@ def h2d_plan(shapes, datas, from_host):
         esize = _element_size(d["fmap_host"])
         nbytes = d["fmap_host"].numel() * esize
         t_dma = nbytes / 50e9 + 1e-4
-        plan.append("dma" if (nbytes <= cap and t_dma < ratio * _zero_copy_seconds(s, esize)) else "zc")
+        t_zc = _zero_copy_seconds(s, esize, d.get("host_layout", "nchw"))
+        plan.append("dma" if (nbytes <= cap and t_dma < ratio * t_zc) else "zc")
     return plan
 
 
@@ -207,7 +222,8 @@ def _prune_layers_ordered(eng, shapes, datas, right0, rank_tol, from_host, to_ho
                 continue
             eng.use_slot(i)
             with torch.cuda.stream(zc_stream):
-                X = eng.patch_gather(d["fmap_host"], d["randx"], d["randy"], s.B, s.P, s.k, s.pad, s.stride, relu=True)
+                X = eng.patch_gather(d["fmap_host"], d["randx"], d["randy"], s.B, s.P, s.k, s.pad, s.stride, relu=True,
+                                     layout=d.get("host_layout", "nchw"))
                 _mark(trace, s.name, "zc_done")
                 ev = torch.cuda.Event()
                 ev.record()
@@ -220,7 +236,7 @@ def _prune_layers_ordered(eng, shapes, datas, right0, rank_tol, from_host, to_ho
             if stream is not None:
                 stream.wait_stream(main)
             X = None
-            layout = "nchw"
+            layout = d.get("host_layout", "nchw")  # of fmap_host, and of its staged copy in HBM
             if pre[i] is not None:
                 kind, obj, ev = pre[i]
                 stream.wait_event(ev)
@@ -237,7 +253,7 @@ def _prune_layers_ordered(eng, shapes, datas, right0, rank_tol, from_host, to_ho
                 fmap = d["fmap_host"]
             else:
                 fmap = d["fmap"]
-                layout = d.get("layout", "nchw")  # host copies keep the reference's NCHW blob order
+                layout = d.get("layout", "nchw")  # HBM layout of fmap
             if X is None:
                 X = eng.patch_gather(fmap, d["randx"], d["randy"], s.B, s.P, s.k, s.pad, s.stride, relu=True,
                                      layout=layout)

@@ -133,13 +133,16 @@ def fmap_nchw(d):
     return d["fmap"].permute(0, 3, 1, 2) if d.get("layout", "nchw") == "nhwc" else d["fmap"]
 
 
-def make_problem_device(shape: LayerShape, seed: int, eng, noise=0.01, pinned_host=False, layout="nchw", dtype=None):
+def make_problem_device(shape: LayerShape, seed: int, eng, noise=0.01, pinned_host=False, layout="nchw", dtype=None,
+                        host_layout="nchw"):
     """Device instance (torch CUDA generator), sized for BASELINE configs (GBs of feature maps).
     feats are produced with the library's own gather + a torch fp64 matmul: this is data
     generation, outside any timed region.
     layout: how the bottom blob sits in HBM.  'nhwc' (channels last, what a device-side forward provider hands over)
-    takes the TMA gather; the VALUES are those of the 'nchw' instance of the same seed.  The pinned host copy
-    (fmap_host) always keeps the reference's NCHW blob order.
+    takes the TMA gather; the VALUES are those of the 'nchw' instance of the same seed.
+    host_layout: how the pinned host copy (fmap_host) is laid out: the reference's NCHW blob order, or 'nhwc'
+    (channels last, what a user offloading a channels_last forward's maps hands over; the same values, and the dict
+    then carries host_layout='nhwc').
     dtype: element type of the feature maps (fmap, fmap_host): None / torch.float32, or torch.bfloat16 /
     torch.float16 as a 16-bit forward pass would hand them over -- drawn in fp32 as for float32, then rounded; the
     targets are computed from the rounded map."""
@@ -167,7 +170,13 @@ def make_problem_device(shape: LayerShape, seed: int, eng, noise=0.01, pinned_ho
     out = dict(fmap=fmap, randx=randx, randy=randy, W2=W2, b2=b2, feats=feats, samples=samples, seeds=seeds,
                layout=layout)
     del X, Y
-    if pinned_host:
+    assert host_layout in ("nchw", "nhwc"), host_layout
+    if pinned_host and host_layout == "nhwc":
+        src = fmap.permute(0, 2, 3, 1)
+        out["fmap_host"] = torch.empty(src.shape, dtype=fmap.dtype, pin_memory=True)
+        out["fmap_host"].copy_(src)
+        out["host_layout"] = "nhwc"
+    elif pinned_host:
         out["fmap_host"] = torch.empty(fmap.shape, dtype=fmap.dtype, pin_memory=True)
         out["fmap_host"].copy_(fmap)
     if layout == "nhwc":

@@ -91,16 +91,19 @@ int cp_gram_kernel_ms(cp_handle_t h, float *ms);
  *   fmap   : nbatch*B images, layout NCHW (B,c,H,W) or NHWC (B,H,W,c), fp32 (cp_patch_gather) or fmap_dtype
  *            CP_F32 | CP_BF16 | CP_F16 (cp_patch_gather_typed; CP_F64 and other codes return CP_ERR_INVALID).
  *            16-bit values are widened exactly to fp32 and the relu is applied after widening, so X is bit for
- *            bit the X of the fp32 map holding the widened values.  Device memory, or -- NCHW --
+ *            bit the X of the fp32 map holding the widened values.  Device memory, or -- NCHW or NHWC --
  *            page-locked host memory mapped under UVA (cudaHostAlloc / pinned torch tensor): the kernel then
  *            reads the sampled windows in place over PCIe with a small persistent grid (the reference keeps
- *            its feature maps in host RAM; only the windows have to cross).
+ *            its feature maps in host RAM; only the windows have to cross).  An NHWC host map is read as
+ *            whole contiguous window rows, with 16-byte loads when c * element size is a multiple of 16
+ *            bytes and the map is 16-byte aligned (csrc/gather_host.cu).
  *            NHWC in device memory with c >= 16, c % 4 == 0 (fp32) or c % 8 == 0 (bf16 / fp16: the 16-byte
  *            stride rule of TMA), and 16-byte aligned fmap / X_out / ldx takes the TMA path
  *            (csrc/gather_tma.cu): one 4-D tensor-map request per k x k x c window, padding taps zero-filled
  *            by the copy engine, the patch row leaves as one bulk store -- 74 % of the HBM copy rate at conv4_x
- *            (NCHW: 24 %; k-float runs cannot be fetched at sector efficiency).  Other NHWC maps take the SIMT
- *            kernel.  Results are bit-identical.
+ *            (NCHW: 24 %; k-float runs cannot be fetched at sector efficiency).  Other NHWC device maps take the
+ *            SIMT kernel.  NHWC maps off the TMA path (host or device) accept kernel_size <= 9; a larger one
+ *            returns CP_ERR_INVALID.  Results are bit-identical.
  *   randx  : nbatch*P sampled output rows   (points_dict[(batch, Y, "randx")])
  *   randy  : nbatch*P sampled output cols
  *   window : rows [stride*x - pad, +k), cols [stride*y - pad, +k) of the bottom
