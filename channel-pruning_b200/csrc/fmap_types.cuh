@@ -15,3 +15,11 @@ __device__ __forceinline__ float cp_widen(__half v) { return __half2float(v); }
 static inline int cp_fmap_esize(int fmap_dtype) {
     return fmap_dtype == CP_F32 ? 4 : (fmap_dtype == CP_BF16 || fmap_dtype == CP_F16) ? 2 : 0;
 }
+
+// Window of a patch gather, with the semantics of PyTorch's Conv2d: output point (x, y) reads the taps
+// (stride_h*x - pad_h + dil_h*i, stride_w*y - pad_w + dil_w*j), i < kh, j < kw, zero outside the map, into column
+// a*kh*kw + i*kw + j.  Only the top / left padding enters: the bottom / right padding only sets the output size.
+// The reference's layers are the square, undilated case (kh = kw = k, one pad, one stride, dilation 1).
+struct cp_window {
+    int kh, kw, pad_h, pad_w, stride_h, stride_w, dil_h, dil_w;
+};

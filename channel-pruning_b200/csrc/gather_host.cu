@@ -2,14 +2,14 @@
 // input path for maps a channels_last forward hands over (cp_patch_gather_typed, layout NHWC, map in page-locked host
 // memory mapped under UVA).
 //
-// Over PCIe a gather costs read requests, not bytes.  In NHWC the in-bounds taps of a window row are one contiguous
-// run of (taps x c) elements, so the reader fetches each run as 16-byte vectors, consecutive threads on consecutive
-// addresses: every 128-byte line of the run is requested once and nearly all of its bytes are used (NCHW: c*k runs of
-// k elements per window).
-// A work unit is one (output row, channel chunk).  Its k*k x ct sub-window is copied by cp.async into a shared-memory
-// stage; while one unit is widened, transposed to the (c, k*k) column order and stored, the copies of the next NS - 1
-// units of the CTA are in flight.  Chunks keep a stage within NHWC_HOST_SMEM / NS bytes whatever c and k (a c = 2048,
-// k = 3 fp32 window is 72 KB).  A small persistent grid strides over the units: the zero-copy gathers run beside other
+// Over PCIe a gather costs read requests, not bytes.  In NHWC the in-bounds taps of an undilated window row are one
+// contiguous run of (taps x c) elements (a dilated row: kw runs of c elements), so the reader fetches each run as
+// 16-byte vectors, consecutive threads on consecutive addresses: every 128-byte line of the run is requested once and
+// nearly all of its bytes are used (NCHW: c*kh runs of kw elements per window).
+// A work unit is one (output row, channel chunk).  Its kh*kw x ct sub-window (cp_window) is copied by cp.async into a
+// shared-memory stage; while one unit is widened, transposed to the (c, kh*kw) column order and stored, the copies of
+// the next NS - 1 units of the CTA are in flight.  Chunks keep a stage within NHWC_HOST_SMEM / NS bytes whatever c and
+// kh*kw <= 81 (a c = 2048, 3 x 3 fp32 window is 72 KB).  A small persistent grid strides over the units: the zero-copy gathers run beside other
 // layers' searches and Grams, which need the SMs.
 // Maps whose channel stride or base address is not a multiple of 16 bytes (c = 3, 5, 12 in fp32; odd c in 16 bit)
 // take plain element loads into the same stages: correct for every c, not tuned.
@@ -23,7 +23,8 @@ constexpr int NHWC_HOST_SMEM = 48 * 1024;  // shared memory of a CTA (all stages
 constexpr int NHWC_HOST_PAD = 16;          // bytes after each tap of a stage: keeps 16-byte alignment, spreads banks
 
 struct NhwcHostGeom {
-    int B, P, c, H, W, k, pad, stride;
+    int B, P, c, H, W;
+    cp_window w;
     int ct;       // channels per chunk (the last chunk may be shorter)
     int nchunk;   // chunks per window
     int tap;      // bytes per tap in a stage: ct * esize + NHWC_HOST_PAD
@@ -44,34 +45,34 @@ __device__ __forceinline__ void nhwc_host_fetch(const T *__restrict__ fmap, cons
     const int64_t r = u / g.nchunk;
     const int a0 = (int)(u - r * g.nchunk) * g.ct;
     const int ct = min(g.ct, g.c - a0);
-    const int k2 = g.k * g.k;
+    const int k2 = g.w.kh * g.w.kw;
     const int64_t bp = r / g.B;
     const int img = (int)(bp / g.P) * g.B + (int)(r % g.B);
-    const int y0 = g.stride * randx[bp] - g.pad;
-    const int x0 = g.stride * randy[bp] - g.pad;
+    const int y0 = g.w.stride_h * randx[bp] - g.w.pad_h;
+    const int x0 = g.w.stride_w * randy[bp] - g.w.pad_w;
     const T *src = fmap + (int64_t)img * g.H * g.W * g.c + a0;
     if (g.vec) {
         constexpr int VE = 16 / sizeof(T);  // elements per copy
         const int nv = ct / VE;
         for (int e = threadIdx.x; e < k2 * nv; e += blockDim.x) {
             const int p = e / nv, j = e - p * nv;
-            const int py = p / g.k, px = p - py * g.k;
-            const int yy = y0 + py, xx = x0 + px;
+            const int py = p / g.w.kw, px = p - py * g.w.kw;
+            const int yy = y0 + py * g.w.dil_h, xx = x0 + px * g.w.dil_w;
             if (yy >= 0 && yy < g.H && xx >= 0 && xx < g.W)
                 nh_cp_async16(stage + p * g.tap + j * 16, src + ((int64_t)yy * g.W + xx) * g.c + j * VE);
         }
     } else {
         for (int e = threadIdx.x; e < k2 * ct; e += blockDim.x) {
             const int p = e / ct, a = e - p * ct;
-            const int py = p / g.k, px = p - py * g.k;
-            const int yy = y0 + py, xx = x0 + px;
+            const int py = p / g.w.kw, px = p - py * g.w.kw;
+            const int yy = y0 + py * g.w.dil_h, xx = x0 + px * g.w.dil_w;
             if (yy >= 0 && yy < g.H && xx >= 0 && xx < g.W)
                 reinterpret_cast<T *>(stage + p * g.tap)[a] = __ldg(src + ((int64_t)yy * g.W + xx) * g.c + a);
         }
     }
 }
 
-// Writes unit u from its stage: column a*k*k + p of the chunk, zero for taps outside the map.
+// Writes unit u from its stage: column a*kh*kw + p of the chunk, zero for taps outside the map.
 template <typename T>
 __device__ __forceinline__ void nhwc_host_store(const int32_t *__restrict__ randx, const int32_t *__restrict__ randy,
                                                 float *__restrict__ X, int64_t ldx, const NhwcHostGeom &g, int64_t u,
@@ -79,15 +80,15 @@ __device__ __forceinline__ void nhwc_host_store(const int32_t *__restrict__ rand
     const int64_t r = u / g.nchunk;
     const int a0 = (int)(u - r * g.nchunk) * g.ct;
     const int ct = min(g.ct, g.c - a0);
-    const int k2 = g.k * g.k;
+    const int k2 = g.w.kh * g.w.kw;
     const int64_t bp = r / g.B;
-    const int y0 = g.stride * randx[bp] - g.pad;
-    const int x0 = g.stride * randy[bp] - g.pad;
+    const int y0 = g.w.stride_h * randx[bp] - g.w.pad_h;
+    const int x0 = g.w.stride_w * randy[bp] - g.w.pad_w;
     float *dst = X + r * ldx + (int64_t)a0 * k2;
     for (int e = threadIdx.x; e < k2 * ct; e += blockDim.x) {
         const int a = e / k2, p = e - a * k2;
-        const int py = p / g.k, px = p - py * g.k;
-        const int yy = y0 + py, xx = x0 + px;
+        const int py = p / g.w.kw, px = p - py * g.w.kw;
+        const int yy = y0 + py * g.w.dil_h, xx = x0 + px * g.w.dil_w;
         float v = 0.f;
         if (yy >= 0 && yy < g.H && xx >= 0 && xx < g.W) v = cp_widen(reinterpret_cast<const T *>(stage + p * g.tap)[a]);
         if (relu) v = fmaxf(v, 0.f);
@@ -125,11 +126,11 @@ patch_gather_nhwc_host(const T *__restrict__ fmap, const int32_t *__restrict__ r
 }  // namespace
 
 // Geometry of the reader for one map: channel chunk and stage sizes for NS stages.  Returns false when one copy per
-// tap does not fit a stage (never for the k <= 9 that cp_patch_gather_typed lets through).
-static bool nhwc_host_geom(NhwcHostGeom &g, const void *fmap, int esize, int B, int P, int c, int H, int W, int k,
-                           int pad, int stride, int ns) {
-    const int k2 = k * k;
-    g.B = B, g.P = P, g.c = c, g.H = H, g.W = W, g.k = k, g.pad = pad, g.stride = stride;
+// tap does not fit a stage (never for the kh*kw <= 81 that cp_patch_gather_conv lets through).
+static bool nhwc_host_geom(NhwcHostGeom &g, const void *fmap, int esize, int B, int P, int c, int H, int W,
+                           const cp_window &w, int ns) {
+    const int k2 = w.kh * w.kw;
+    g.B = B, g.P = P, g.c = c, g.H = H, g.W = W, g.w = w;
     g.vec = (c * esize) % 16 == 0 && ((uintptr_t)fmap & 15) == 0;
     const int ve = g.vec ? 16 / esize : 1;
     int ctmax = (NHWC_HOST_SMEM / ns / k2 - NHWC_HOST_PAD) / esize;
@@ -160,11 +161,11 @@ constexpr int CP_HOST_NHWC_GATHER_CTAS = 32;
 constexpr int CP_HOST_NHWC_STAGES = 2;
 
 int cp_patch_gather_nhwc_host(const void *fmap, int fmap_dtype, int nbatch, int B, int c, int H, int W,
-                              const int32_t *randx, const int32_t *randy, int P, int k, int pad, int stride, int relu,
+                              const int32_t *randx, const int32_t *randy, int P, const cp_window &w, int relu,
                               float *X_out, int64_t ldx, cudaStream_t stream) {
     NhwcHostGeom g;
-    CP_REQUIRE(nhwc_host_geom(g, fmap, cp_fmap_esize(fmap_dtype), B, P, c, H, W, k, pad, stride, CP_HOST_NHWC_STAGES),
-               "cp_patch_gather: kernel_size %d too large for the NHWC host reader", k);
+    CP_REQUIRE(nhwc_host_geom(g, fmap, cp_fmap_esize(fmap_dtype), B, P, c, H, W, w, CP_HOST_NHWC_STAGES),
+               "cp_patch_gather: kernel_size %dx%d too large for the NHWC host reader", w.kh, w.kw);
     const int64_t rows = (int64_t)nbatch * P * B;
     if (fmap_dtype == CP_F32)
         launch_nhwc_host<CP_HOST_NHWC_STAGES>((const float *)fmap, g, rows, randx, randy, relu, X_out, ldx,

@@ -1,16 +1,18 @@
 // Sparse-point im2col on NHWC feature maps, TMA in / TMA out -- the HBM-roofline path of cp_patch_gather
 // (replaces Net.extract_XY, reference lib/net.py:534-684, + the relu of lib/net.py:1720).
 //
-// One sampled output point needs a k x k x c window of the bottom blob.  In NHWC that window is k runs of k*c
-// contiguous floats (6 KB at c = 512): a 4-D tensor map over (c, W, H, image) with box (c_box, k, k, 1) lets ONE
-// cp.async.bulk.tensor request fetch it, zero-filling the taps that fall into the padding (out-of-range coordinates,
-// net.py:631-632), and the finished patch row (K = c k k contiguous floats of X) leaves through a bulk shared->global
-// copy.  Persistent CTAs (as many per SM as shared memory allows: the latency of one row -- TMA flight, two CTA-wide
+// One sampled output point needs a kh x kw x c window of the bottom blob (cp_window).  In NHWC that window is kh runs
+// of kw*c contiguous floats (6 KB at c = 512, 3 x 3): a 4-D tensor map over (c, W, H, image) with box
+// (c_box, (kw-1)*dil_w+1, (kh-1)*dil_h+1, 1) and traversal strides (1, dil_w, dil_h, 1) lets ONE cp.async.bulk.tensor
+// request fetch it -- the copy engine delivers ceil(box / stride) = kw x kh taps per channel, so a dilated window lands
+// as densely as an undilated one -- zero-filling the taps that fall into the padding (out-of-range coordinates,
+// net.py:631-632), and the finished patch row (K = c kh kw contiguous floats of X) leaves through a bulk
+// shared->global copy.  Persistent CTAs (as many per SM as shared memory allows: the latency of one row -- TMA flight, two CTA-wide
 // hand-offs, the transposition -- is hidden by the other CTAs of the SM) each keep a ring of windows in flight:
 //     producer warp     the 32 lanes prefetch the sampled coordinates of the next 32 rows (one global-load latency per
 //                       32 rows instead of per row); one lane arms the mbarrier and issues the TMA loads (ring of NS stages)
-//     128 consumers     [tap][channel] -> [channel][tap] (the reference's column order a*k*k + p) with the ReLU folded in,
-//                       conflict-free both ways (lanes walk channels; the tap stride k*k is odd)
+//     128 consumers     [tap][channel] -> [channel][tap] (the reference's column order a*kh*kw + p) with the ReLU folded
+//                       in, conflict-free both ways when kh*kw is odd (lanes walk channels, the tap stride is kh*kw)
 //     one consumer      bulk store of the row, two rows in flight
 // Bytes: the window is read once and the row written once -- 8 N K bytes, the algorithmic figure of SURVEY.md 8(d).
 // Bound: HBM.
@@ -32,7 +34,7 @@ struct GtParams {
     const int32_t *randx, *randy;
     float *X;
     int64_t ldx, rows;
-    int B, P, c, k, pad, stride, relu, cbox, nbox, nstage;
+    int B, P, c, k2, pad_h, pad_w, stride_h, stride_w, relu, cbox, nbox, nstage;
     int box_f, stage_f, out_f;  // strides in map elements (box, stage) and floats (out); 128-byte multiples each
 };
 
@@ -70,11 +72,11 @@ __device__ __forceinline__ void g_bulk_store(void *gdst, uint32_t ssrc, uint32_t
 }
 __device__ __forceinline__ void g_cons_barrier() { asm volatile("bar.sync 1, %0;" ::"n"(GT_CONS) : "memory"); }
 
-template <typename T, int K2>  // map element type; k*k known at compile time (1, 9, 25) or 0
+template <typename T, int K2>  // map element type; kh*kw known at compile time (1, 9, 25) or 0
 __global__ void __launch_bounds__(GT_THREADS)
 patch_gather_nhwc_tma(const __grid_constant__ CUtensorMap map, const GtParams P) {
     extern __shared__ __align__(128) unsigned char gsm_raw[];
-    const int k2 = K2 > 0 ? K2 : P.k * P.k, K = P.c * k2;
+    const int k2 = K2 > 0 ? K2 : P.k2, K = P.c * k2;
     const uint32_t stage_bytes = (uint32_t)K * (uint32_t)sizeof(T), row_bytes = (uint32_t)K * 4u;
     // layout: [nstage][K] input windows ([box][tap][c_box], type T), [GT_OUT][K] fp32 output rows, mbarriers
     unsigned char *base = (unsigned char *)(((uintptr_t)gsm_raw + 127) & ~(uintptr_t)127);
@@ -106,8 +108,8 @@ patch_gather_nhwc_tma(const __grid_constant__ CUtensorMap map, const GtParams P)
                 const int img_in_batch = (int)(r % P.B);
                 const int64_t bp = r / P.B;  // batch * P + point
                 const int batch = (int)(bp / P.P);
-                y0 = P.stride * P.randx[bp] - P.pad;  // window origin, rows  (feat[:,:,x,y]: x indexes H)
-                x0 = P.stride * P.randy[bp] - P.pad;
+                y0 = P.stride_h * P.randx[bp] - P.pad_h;  // window origin, rows  (feat[:,:,x,y]: x indexes H)
+                x0 = P.stride_w * P.randy[bp] - P.pad_w;
                 img = batch * P.B + img_in_batch;
             }
             const int64_t left = (P.rows - rb + step - 1) / step;
@@ -171,6 +173,14 @@ patch_gather_nhwc_tma(const __grid_constant__ CUtensorMap map, const GtParams P)
 
 inline size_t gt_round128(size_t b) { return (b + 127) & ~(size_t)127; }
 
+// Elements one tiled TMA request delivers to shared memory: ceil(boxDim[i] / elementStrides[i]) per dimension (the
+// rule of the cuTensorMapEncodeTiled documentation)
+inline size_t gt_box_elems(const cuuint32_t box[4], const cuuint32_t estr[4]) {
+    size_t n = 1;
+    for (int i = 0; i < 4; ++i) n *= (box[i] + estr[i] - 1) / estr[i];
+    return n;
+}
+
 typedef CUresult (*encode_fn_t)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
                                 const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
                                 CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -178,12 +188,14 @@ typedef CUresult (*encode_fn_t)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, 
 }  // namespace
 
 template <typename T>
-static int gt_launch(cp_handle_t h, const CUtensorMap &map, const GtParams &Pm, int k, size_t smem, int per_sm,
+static int gt_launch(cp_handle_t h, const CUtensorMap &map, const GtParams &Pm, size_t smem, int per_sm,
                      cudaStream_t stream) {
-    auto kern = k == 3 ? patch_gather_nhwc_tma<T, 9> : k == 1 ? patch_gather_nhwc_tma<T, 1>
-              : k == 5 ? patch_gather_nhwc_tma<T, 25> : patch_gather_nhwc_tma<T, 0>;
+    // the consumers only see the number of taps: a dilated 3 x 3 window takes the 3 x 3 instantiation
+    const int k2 = Pm.k2;
+    auto kern = k2 == 9 ? patch_gather_nhwc_tma<T, 9> : k2 == 1 ? patch_gather_nhwc_tma<T, 1>
+              : k2 == 25 ? patch_gather_nhwc_tma<T, 25> : patch_gather_nhwc_tma<T, 0>;
     static cp_per_device_flag configured[4];  // one set per element type (one per instantiation of gt_launch)
-    const int which = k == 3 ? 0 : k == 1 ? 1 : k == 5 ? 2 : 3;
+    const int which = k2 == 9 ? 0 : k2 == 1 ? 1 : k2 == 25 ? 2 : 3;
     if (bool *done = configured[which].slot(); !*done) {
         CP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
         *done = true;
@@ -202,9 +214,16 @@ static int gt_cbox(int c, int esize) {
     return 0;
 }
 
-// true when the TMA path applies (device memory, 16-byte rules); the caller falls back to the SIMT kernel otherwise
-bool cp_gather_tma_eligible(const void *fmap, int esize, int c, int k, float *X_out, int64_t ldx) {
-    if (c % (16 / esize) || c < 16 || k > 16) return false;
+// Traversal strides of a tensor map are at most 8 and box extents at most 256 (cuTensorMapEncodeTiled)
+constexpr int GT_MAX_DIL = 8, GT_MAX_SPAN = 256;
+
+// true when the TMA path applies (device memory, 16-byte rules, dilation <= 8, window spans <= 256, extents <= 16);
+// the caller falls back to the SIMT kernel otherwise
+bool cp_gather_tma_eligible(const void *fmap, int esize, int c, const cp_window &g, float *X_out, int64_t ldx) {
+    if (c % (16 / esize) || c < 16 || g.kh > 16 || g.kw > 16) return false;
+    if (g.dil_h > GT_MAX_DIL || g.dil_w > GT_MAX_DIL) return false;
+    if ((g.kh - 1) * g.dil_h + 1 > GT_MAX_SPAN || (g.kw - 1) * g.dil_w + 1 > GT_MAX_SPAN) return false;
+    const int k2 = g.kh * g.kw;
     if (((uintptr_t)fmap & 15) || ((uintptr_t)X_out & 15) || (ldx % 4)) return false;
     cudaPointerAttributes pa;
     if (cudaPointerGetAttributes(&pa, fmap) != cudaSuccess || pa.type != cudaMemoryTypeDevice) {
@@ -214,13 +233,13 @@ bool cp_gather_tma_eligible(const void *fmap, int esize, int c, int k, float *X_
     const int cbox = gt_cbox(c, esize);
     if (!cbox) return false;
     // a window stage and an output row; for fp32 the stage is never smaller than the row
-    const size_t row = gt_round128((size_t)cbox * k * k * esize) * (c / cbox);
-    const size_t out_b = gt_round128((size_t)c * k * k * 4);
+    const size_t row = gt_round128((size_t)cbox * k2 * esize) * (c / cbox);
+    const size_t out_b = gt_round128((size_t)c * k2 * 4);
     return 2 * row + GT_OUT * (row > out_b ? row : out_b) + 1024 <= 200 * 1024;  // at least two input stages in one CTA
 }
 
 int cp_patch_gather_tma(cp_handle_t h, const void *fmap, int fmap_dtype, int nbatch, int B, int c, int H, int W,
-                        const int32_t *randx, const int32_t *randy, int P, int k, int pad, int stride, int relu,
+                        const int32_t *randx, const int32_t *randy, int P, const cp_window &g, int relu,
                         float *X_out, int64_t ldx, cudaStream_t stream) {
     if (!h->tmap_encode) {
         void *fn = nullptr;
@@ -235,8 +254,10 @@ int cp_patch_gather_tma(cp_handle_t h, const void *fmap, int fmap_dtype, int nba
     CUtensorMap map;
     const cuuint64_t dims[4] = {(cuuint64_t)c, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)nimg};
     const cuuint64_t strides[3] = {(cuuint64_t)c * esize, (cuuint64_t)W * c * esize, (cuuint64_t)H * W * c * esize};
-    const cuuint32_t box[4] = {(cuuint32_t)cbox, (cuuint32_t)k, (cuuint32_t)k, 1};
-    const cuuint32_t estr[4] = {1, 1, 1, 1};
+    // the box spans the dilated window; the traversal strides pick its kw x kh taps, which land densely
+    const cuuint32_t box[4] = {(cuuint32_t)cbox, (cuuint32_t)((g.kw - 1) * g.dil_w + 1),
+                               (cuuint32_t)((g.kh - 1) * g.dil_h + 1), 1};
+    const cuuint32_t estr[4] = {1, (cuuint32_t)g.dil_w, (cuuint32_t)g.dil_h, 1};
     const CUtensorMapDataType dt = fmap_dtype == CP_BF16  ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
                                    : fmap_dtype == CP_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
                                                           : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
@@ -247,10 +268,17 @@ int cp_patch_gather_tma(cp_handle_t h, const void *fmap, int fmap_dtype, int nba
     GtParams Pm{};
     Pm.randx = randx; Pm.randy = randy; Pm.X = X_out; Pm.ldx = ldx;
     Pm.rows = (int64_t)nbatch * P * B;
-    Pm.B = B; Pm.P = P; Pm.c = c; Pm.k = k; Pm.pad = pad; Pm.stride = stride; Pm.relu = relu;
+    const int k2 = g.kh * g.kw;
+    Pm.B = B; Pm.P = P; Pm.c = c; Pm.k2 = k2; Pm.relu = relu;
+    Pm.pad_h = g.pad_h; Pm.pad_w = g.pad_w; Pm.stride_h = g.stride_h; Pm.stride_w = g.stride_w;
     Pm.cbox = cbox; Pm.nbox = c / cbox;
-    const size_t box_b = gt_round128((size_t)cbox * k * k * esize), row = box_b * Pm.nbox;
-    const size_t out_b = gt_round128((size_t)c * k * k * 4);
+    // Bytes the copy engine delivers per box, hence what expect_tx must announce (the kernel arms c * k2 * esize per
+    // window): ceil(box[i] / estr[i]) elements per dimension, i.e. cbox x kw x kh x 1 (gt_box_elems).
+    const size_t box_b = gt_round128(gt_box_elems(box, estr) * esize), row = box_b * Pm.nbox;
+    if (gt_box_elems(box, estr) != (size_t)cbox * k2)
+        CP_FAIL(CP_ERR_CUDA, "cp_patch_gather: TMA box delivers %zu elements, the window has %zu",
+                gt_box_elems(box, estr), (size_t)cbox * k2);
+    const size_t out_b = gt_round128((size_t)c * k2 * 4);
     // CTAs per SM: as many as fit with >= 2 input stages each (up to 4), then the stages fill what is left.
     // conv4_x (c = 512, k = 3): fp32 stage 18 KB, row 18 KB -> 2 CTAs x 3 stages; 16-bit stage 9 KB, row 18 KB ->
     // 3 CTAs x 3 stages (the fp32 output rows then take most of the budget)
@@ -262,7 +290,7 @@ int cp_patch_gather_tma(cp_handle_t h, const void *fmap, int fmap_dtype, int nba
     Pm.nstage = nstage;
     Pm.box_f = (int)(box_b / esize); Pm.stage_f = (int)(row / esize); Pm.out_f = (int)(out_b / 4);
     const size_t smem = (size_t)nstage * row + GT_OUT * out_b + 2 * nstage * 8 + 256;
-    if (fmap_dtype == CP_BF16) return gt_launch<__nv_bfloat16>(h, map, Pm, k, smem, per_sm, stream);
-    if (fmap_dtype == CP_F16) return gt_launch<__half>(h, map, Pm, k, smem, per_sm, stream);
-    return gt_launch<float>(h, map, Pm, k, smem, per_sm, stream);
+    if (fmap_dtype == CP_BF16) return gt_launch<__nv_bfloat16>(h, map, Pm, smem, per_sm, stream);
+    if (fmap_dtype == CP_F16) return gt_launch<__half>(h, map, Pm, smem, per_sm, stream);
+    return gt_launch<float>(h, map, Pm, smem, per_sm, stream);
 }

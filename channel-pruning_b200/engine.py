@@ -35,6 +35,14 @@ GRAM_FP64, GRAM_3XTF32 = 0, 1
 FMAP_DTYPES = {torch.float32: 0, torch.bfloat16: 2, torch.float16: 3}
 
 
+def conv_pair(v):
+    """(h, w) of a Conv2d-style argument given as an int or a pair (kernel_size, padding, stride, dilation)."""
+    if isinstance(v, (tuple, list)):
+        assert len(v) == 2, v
+        return int(v[0]), int(v[1])
+    return int(v), int(v)
+
+
 def fmap_dtype_code(dtype):
     """The C ABI code of a feature-map dtype; TypeError for a type the gathers do not read."""
     code = FMAP_DTYPES.get(dtype)
@@ -230,10 +238,13 @@ class Engine:
         return torch.empty(*shape, dtype=dtype, device=self.device)
 
     # ------------------------------------------------------------------ kernels
-    def patch_gather(self, fmap, randx, randy, B, P, k, pad, stride, relu=True, layout="nchw", out=None):
+    def patch_gather(self, fmap, randx, randy, B, P, k, pad, stride, relu=True, layout="nchw", out=None, dilation=1):
         """fmap: (nbatch*B, c, H, W) [nchw] or (nbatch*B, H, W, c) [nhwc], float32 / bfloat16 / float16, on device
-        or in pinned host memory (read in place over PCIe); randx/randy: (nbatch, P) int32 on device.  Returns X (nbatch*P*B, c*k*k)
-        fp32 -- 16-bit maps are widened exactly, so X equals the X of fmap.float()."""
+        or in pinned host memory (read in place over PCIe); randx/randy: (nbatch, P) int32 on device.  Returns X (nbatch*P*B, c*kh*kw)
+        fp32 -- 16-bit maps are widened exactly, so X equals the X of fmap.float().
+        k, pad, stride, dilation: an int or an (h, w) pair, with the meaning of torch.nn.Conv2d's arguments (pad: the
+        top / left padding; the sampled points already respect the output size).  Columns are in F.unfold's order.
+        All ints with dilation 1 is the reference's window, which must be odd (an even square kernel is (k, k))."""
         dt = fmap_dtype_code(fmap.dtype)
         assert fmap.is_contiguous()
         nimg = fmap.shape[0]
@@ -245,14 +256,18 @@ class Engine:
             H, W, c = fmap.shape[1], fmap.shape[2], fmap.shape[3]
         assert randx.dtype == torch.int32 and randx.numel() == nbatch * P and randx.is_contiguous()
         assert randy.dtype == torch.int32 and randy.numel() == nbatch * P and randy.is_contiguous()
-        rows, K = nbatch * P * B, c * k * k
+        (kh, kw), (ph, pw), (sh, sw), (dh, dw) = (conv_pair(v) for v in (k, pad, stride, dilation))
+        rows, K = nbatch * P * B, c * kh * kw
         if out is None:
             out = self.empty(rows, K, dtype=torch.float32)
         assert out.shape == (rows, K) and out.dtype == torch.float32 and out.stride(1) == 1
-        self._call(self.lib.cp_patch_gather_typed(self.h, self._p(fmap, "const void*"), dt, nbatch, B, c, H, W,
-                                                  _LAYOUTS[layout], self._p(randx, "const int32_t*"),
-                                                  self._p(randy, "const int32_t*"), P, k, pad, stride, int(bool(relu)),
-                                                  self._p(out, "float*"), out.stride(0), self._s()))
+        args = (self.h, self._p(fmap, "const void*"), dt, nbatch, B, c, H, W, _LAYOUTS[layout],
+                self._p(randx, "const int32_t*"), self._p(randy, "const int32_t*"), P)
+        tail = (int(bool(relu)), self._p(out, "float*"), out.stride(0), self._s())
+        if all(isinstance(v, (int, np.integer)) for v in (k, pad, stride, dilation)) and dilation == 1:
+            self._call(self.lib.cp_patch_gather_typed(*args, kh, ph, sh, *tail))
+        else:
+            self._call(self.lib.cp_patch_gather_conv(*args, kh, kw, ph, pw, sh, sw, dh, dw, *tail))
         return out
 
     def point_gather(self, fmap, randx, randy, B, P, layout="nchw", out=None):

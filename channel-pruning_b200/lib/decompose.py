@@ -69,6 +69,7 @@ def dictionary(X, W2, Y, alpha=1e-4, rank=None, DEBUG=0, B2=None, rank_tol=.1, v
 
     X: (N, c, h, w)   W2: (n, c, h, w)   Y: (N, n)   rank: channels to keep
     returns (idxs bool[c], newW2 (n, c', h, w) float64, newB2 (n,) float64)
+    h != w (a 1 x 7 or 3 x 1 layer) is accepted: columns are (c, h, w) in that order, as F.unfold gives them.
     or, with DEBUG, (newX, newW2, newB2) (decompose.py:629-632).
 
     Reference behaviour that is kept on purpose:
@@ -77,7 +78,8 @@ def dictionary(X, W2, Y, alpha=1e-4, rank=None, DEBUG=0, B2=None, rank_tol=.1, v
         further global draw per Lasso.fit for its coordinate order (sklearn _cd_fast)
       * alpha search starts at cfgs.alpha and stores the final alpha back (:491, :627);
         with rank == c the LASSO is skipped and cfgs.alpha becomes the *argument* (:487, :627)
-      * square kernels assumed: w = h (:401-402)
+      * the reference assumes square kernels, w = h (:401-402); here w is read from X.shape[3].  Square inputs draw
+        the same RNG values and give the same results as the reference
     Deviation: the reference's unguarded ``while True`` loops (:502, :516) are capped at
     64 probes; hitting the cap raises RuntimeError instead of spinning forever.
     """
@@ -85,14 +87,13 @@ def dictionary(X, W2, Y, alpha=1e-4, rank=None, DEBUG=0, B2=None, rank_tol=.1, v
             dcfgs.dic.debug or dcfgs.fc_ridge or dcfgs.nonlinear_fc or dcfgs.nofc:
         raise NotImplementedError("only the `train.py -action c3` configuration of dictionary() is implemented")
     eng = get_engine()
-    N, c, h = X.shape[0], X.shape[1], X.shape[2]
-    w = h
+    N, c, h, w = X.shape[0], X.shape[1], X.shape[2], X.shape[3]
     n = W2.shape[0]
     assert tuple(X.shape) == (N, c, h, w) and tuple(W2.shape) == (n, c, h, w) and tuple(Y.shape) == (N, n)
     Xd = _dev_f32(X, eng).reshape(N, c * h * w)
     W2m = _dev_f32(W2, eng).reshape(n, c * h * w)
     Yd = _dev_y(Y, eng)
-    idxs, Wd, bd = _dictionary_device(eng, Xd, W2m, Yd, None, c, h, rank, alpha)
+    idxs, Wd, bd = _dictionary_device(eng, Xd, W2m, Yd, None, c, h * w, rank, alpha)
     rank = int(idxs.sum())
     newW2 = Wd.cpu().numpy().reshape((n, rank, h, w))
     newB2 = bd.cpu().numpy()
@@ -102,13 +103,12 @@ def dictionary(X, W2, Y, alpha=1e-4, rank=None, DEBUG=0, B2=None, rank_tol=.1, v
     return idxs, newW2, newB2
 
 
-def _dictionary_device(eng, Xd, W2m, Yd, y_bias, c, h, rank, alpha=1e-4):
-    """Body of ``dictionary`` on device buffers: Xd (N, c*h*h) fp32 in (c,kh,kw) column order,
-    W2m (n, c*h*h) fp32, Yd (N, n) fp32|fp64 with optional fp32 ``y_bias`` subtracted exactly.
+def _dictionary_device(eng, Xd, W2m, Yd, y_bias, c, k2, rank, alpha=1e-4):
+    """Body of ``dictionary`` on device buffers: Xd (N, c*k2) fp32 in (c,kh,kw) column order (k2 = kh*kw taps per
+    channel), W2m (n, c*k2) fp32, Yd (N, n) fp32|fp64 with optional fp32 ``y_bias`` subtracted exactly.
     Returns (idxs numpy bool[c], W (n, K') fp64 device, b (n,) fp64 device)."""
     rank_tol = dcfgs.dic.rank_tol  # :393
     N = Xd.shape[0]
-    k2 = h * h
     S = min(400, N // 20)
     samples = np.random.randint(0, N, S)  # :425 -- consumed even when rank == c, like the reference
     info = {"samples": samples, "probes": [], "alpha": alpha}

@@ -35,7 +35,7 @@ import torch.nn.functional as F
 from . import cfgs
 from .cfgs import c as dcfgs
 from .decompose import ITQ_decompose, VH_decompose, _dictionary_device
-from ..engine import get_engine
+from ..engine import conv_pair, get_engine
 
 
 def underline(*parts):
@@ -44,13 +44,21 @@ def underline(*parts):
 
 
 class ConvSpec:
-    """What the reference reads from the prototxt for a Convolution layer (net.py:542-553)."""
+    """What the reference reads from the prototxt for a Convolution layer (net.py:542-553).
+    kernel_size, pad, stride and dilation are ints or (h, w) pairs with the meaning of torch.nn.Conv2d's arguments
+    (groups == 1): rectangular kernels such as Inception's 1 x 7, per-axis padding and dilated layers such as those
+    of DeepLabV3's backbone.  The reference's layers are square, odd and undilated."""
 
-    def __init__(self, name, bottom, num_output, kernel_size=3, pad=1, stride=1, pool_after=False):
+    def __init__(self, name, bottom, num_output, kernel_size=3, pad=1, stride=1, pool_after=False, dilation=1):
         self.name, self.bottom = name, bottom
         self.num_output = num_output
-        self.kernel_size, self.pad, self.stride = kernel_size, pad, stride
+        self.kernel_size, self.pad, self.stride, self.dilation = kernel_size, pad, stride, dilation
         self.pool_after = pool_after  # a 2x2/2 max-pool follows the ReLU (VGG)
+
+    @property
+    def kernel_hw(self):
+        """(kh, kw)"""
+        return conv_pair(self.kernel_size)
 
 
 class ConvStackForward:
@@ -77,7 +85,7 @@ class ConvStackForward:
         for spec in net._specs:
             w = net._w[spec.name].to(self.dtype)
             b = net._b[spec.name].to(self.dtype)
-            y = F.conv2d(blobs[spec.bottom], w, b, stride=spec.stride, padding=spec.pad)
+            y = F.conv2d(blobs[spec.bottom], w, b, stride=spec.stride, padding=spec.pad, dilation=spec.dilation)
             blobs[spec.name] = y
             r = F.relu(y)
             blobs[spec.name + "_relu"] = r
@@ -286,21 +294,23 @@ class Net:
                 self.forward(upto=upto)[X].contiguous()
             B, c = blob.shape[0], blob.shape[1]
             if out is None:
-                out = eng.empty(nBatches * P * B, c * spec.kernel_size ** 2, dtype=torch.float32)
+                kh, kw = spec.kernel_hw
+                out = eng.empty(nBatches * P * B, c * kh * kw, dtype=torch.float32)
             rx = torch.as_tensor(np.asarray(pd[(batch, Y, "randx")], dtype=np.int32), device=eng.device)
             ry = torch.as_tensor(np.asarray(pd[(batch, Y, "randy")], dtype=np.int32), device=eng.device)
             eng.patch_gather(blob, rx, ry, B, P, spec.kernel_size, spec.pad, spec.stride, relu=relu,
-                             out=out[batch * P * B:(batch + 1) * P * B])
+                             out=out[batch * P * B:(batch + 1) * P * B], dilation=spec.dilation)
         return out
 
     def extract_XY(self, X, Y, DEBUG=False, w1=None):
-        """Returns the (N*k*k, c) float64 matrix of the reference (rows (sample, kh, kw))."""
+        """Returns the (N*kh*kw, c) float64 matrix of the reference (rows (sample, kh, kw)); kh, kw and the rest of the
+        window are those of the consumer Y."""
         assert w1 is None, "the w1 branch (net.py:544-548) is not part of the c3 path"
-        k = self._spec[Y].kernel_size
+        kh, kw = self._spec[Y].kernel_hw
         Xd = self._extract_X_device(X, Y, relu=False)
         N = Xd.shape[0]
-        c = Xd.shape[1] // (k * k)
-        out = Xd.view(N, c, k * k).permute(0, 2, 1).reshape(N * k * k, c)
+        c = Xd.shape[1] // (kh * kw)
+        out = Xd.view(N, c, kh * kw).permute(0, 2, 1).reshape(N * kh * kw, c)
         return out.cpu().numpy().astype(np.float64)
 
     # ---- dictionary_kernel, net.py:1685-1735 (VGG branch: relu on X, resY = 0)
@@ -309,14 +319,14 @@ class Net:
             raise NotImplementedError("ResNet/Xception residual branches (net.py:1716-1719) are not implemented")
         Xd = self._extract_X_device(X_name, Y_name, relu=True)  # :1698 + :1720
         W2 = self._w[Y_name]
-        n, c, h = W2.shape[0], W2.shape[1], W2.shape[-1]
+        n, c, kh, kw = W2.shape
         feats = self._feats_dev[Y_name]
         bias = self._b[Y_name]
         y_bias = bias if feats.dtype == torch.float32 else None
         Yd = feats if y_bias is not None else feats - bias.to(torch.float64)
-        idxs, Wd, bd = _dictionary_device(self.eng, Xd, W2.reshape(n, c * h * h), Yd, y_bias, c, h, d_prime)
+        idxs, Wd, bd = _dictionary_device(self.eng, Xd, W2.reshape(n, c * kh * kw), Yd, y_bias, c, kh * kw, d_prime)
         rank = int(idxs.sum())
-        return idxs, Wd.cpu().numpy().reshape(n, rank, h, h), bd.cpu().numpy()
+        return idxs, Wd.cpu().numpy().reshape(n, rank, kh, kw), bd.cpu().numpy()
 
     # ---- R3, net.py:1292-1471
     def R3(self):

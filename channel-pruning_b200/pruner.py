@@ -18,7 +18,7 @@ import time
 import numpy as np
 import torch
 
-from .engine import Engine, ls_dual, settle_ls, window
+from .engine import Engine, conv_pair, ls_dual, settle_ls, window
 
 
 # ---------------------------------------------------------------------------- assignment
@@ -142,17 +142,29 @@ ZC_NHWC_LINES_PER_S = 7.1e7
 
 
 def zero_copy_lines(s, esize=4, layout="nchw"):
-    """128-byte lines the in-place gather touches in host memory (esize: bytes per map element).
-    nchw: c*k runs of k elements per window; the k rows of a channel are W*esize bytes apart.
-    nhwc: k runs of k*c*esize contiguous bytes per window, plus one line per run when the pixel stride c*esize is
-    not a multiple of 128 bytes (a run may then start inside a line).  An upper bound for a map whose base is
-    128-byte aligned: clipping at the border only removes lines."""
+    """128-byte lines the in-place gather touches in host memory (esize: bytes per map element), for a window of
+    kh x kw taps with dilation (dil_h, dil_w) (s.kh, s.kw, s.dilation; a shape with only s.k is square, undilated).
+    nchw: c*kh rows of kw taps per window, each row counted as the lines its taps span (one for the reference's
+    k <= 9 rows); the rows of a channel are dil_h*W*esize bytes apart.
+    nhwc: kh window rows; an undilated row is one run of kw*c*esize contiguous bytes, a dilated one kw runs of
+    c*esize bytes (or, if fewer, the lines of the span from its first tap to its last); plus one line per run when the
+    pixel stride c*esize is not a multiple of 128 bytes (a run may then start inside a line).  An upper bound for a
+    map whose base is 128-byte aligned: clipping at the border only removes lines.
+    Square, undilated windows give the counts the transfer rates ZC_LINES_PER_S and ZC_NHWC_LINES_PER_S were
+    measured with."""
+    kh, kw = getattr(s, "kh", s.k), getattr(s, "kw", s.k)
+    dh, dw = conv_pair(getattr(s, "dilation", 1))
+    span_w = (kw - 1) * dw + 1  # elements from the first tap of a window row to its last
     if layout == "nhwc":
-        run = s.k * s.c * esize
-        per_run = -(-run // 128) + (1 if (s.c * esize) % 128 else 0)
-        return s.N * s.k * per_run
+        tail = 1 if (s.c * esize) % 128 else 0
+        per_row = -(-span_w * s.c * esize // 128) + tail
+        if dw > 1:
+            per_row = min(per_row, kw * (-(-s.c * esize // 128) + tail))
+        return s.N * kh * per_row
     row = s.W * esize if hasattr(s, "W") else esize * 64
-    lines = min(s.k, -(-((s.k - 1) * row + s.k * esize) // 128) + 1) if s.k > 1 else 1
+    per_row = min(kw, -(-span_w * esize // 128))
+    span = (kh - 1) * dh * row + span_w * esize
+    lines = min(kh * per_row, -(-span // 128) + 1) if kh * kw > 1 else 1
     return s.N * s.c * lines
 
 
@@ -222,8 +234,8 @@ def _prune_layers_ordered(eng, shapes, datas, right0, rank_tol, from_host, to_ho
                 continue
             eng.use_slot(i)
             with torch.cuda.stream(zc_stream):
-                X = eng.patch_gather(d["fmap_host"], d["randx"], d["randy"], s.B, s.P, s.k, s.pad, s.stride, relu=True,
-                                     layout=d.get("host_layout", "nchw"))
+                X = eng.patch_gather(d["fmap_host"], d["randx"], d["randy"], s.B, s.P, relu=True,
+                                     layout=d.get("host_layout", "nchw"), **s.conv_args())
                 _mark(trace, s.name, "zc_done")
                 ev = torch.cuda.Event()
                 ev.record()
@@ -255,15 +267,15 @@ def _prune_layers_ordered(eng, shapes, datas, right0, rank_tol, from_host, to_ho
                 fmap = d["fmap"]
                 layout = d.get("layout", "nchw")  # HBM layout of fmap
             if X is None:
-                X = eng.patch_gather(fmap, d["randx"], d["randy"], s.B, s.P, s.k, s.pad, s.stride, relu=True,
-                                     layout=layout)
+                X = eng.patch_gather(fmap, d["randx"], d["randy"], s.B, s.P, relu=True, layout=layout,
+                                     **s.conv_args())
             W2m = d["W2"].reshape(s.n, s.K)
             if s.rank == s.c:
                 g_full = eng.gram(X, d["feats"], y_bias=d["b2"])
                 res = None
                 host = None
             else:
-                g_full, res = eng.select_channels_async(X, W2m, d["feats"], d["b2"], d["samples"], s.c, s.k * s.k,
+                g_full, res = eng.select_channels_async(X, W2m, d["feats"], d["b2"], d["samples"], s.c, s.k2,
                                                         s.rank, rank_tol, right0, d["seeds"])
                 host = (eng.pinned(("scal", i), (4,), torch.float64), eng.pinned(("idxs", i), (s.c,), torch.uint8))
                 host[0].copy_(res.scalars, non_blocking=True)
@@ -299,7 +311,7 @@ def _prune_layers_ordered(eng, shapes, datas, right0, rank_tol, from_host, to_ho
             r.alpha, r.nprobe = float(scal[0]), int(scal[1])
         ctx = torch.cuda.stream(stream) if stream is not None else _null()
         with eng.slot_lock(i), ctx:  # layers that share a slot (more layers than streams) are issued one after the other
-            W, b, info, stat = eng.reconstruct_async(g_full, X, d["feats"], d["b2"], r.idxs, s.k * s.k)
+            W, b, info, stat = eng.reconstruct_async(g_full, X, d["feats"], d["b2"], r.idxs, s.k2)
             chk = (eng.pinned(("lsinfo", i), (1,), torch.int32), eng.pinned(("lsstat", i), (1,), torch.float64))
             chk[0].copy_(info, non_blocking=True)
             chk[1].copy_(stat, non_blocking=True)
@@ -308,7 +320,7 @@ def _prune_layers_ordered(eng, shapes, datas, right0, rank_tol, from_host, to_ho
             ev_ls.record()
             _mark(trace, s.name, "ls_done")
         r.probes = res
-        r.info = {"mode": g_full["mode"], "dual": ls_dual(g_full["N"], r.idxs, s.k * s.k)}
+        r.info = {"mode": g_full["mode"], "dual": ls_dual(g_full["N"], r.idxs, s.k2)}
         out[i] = r
         return (i, chk, ev_ls)
 
@@ -335,7 +347,7 @@ def _prune_layers_ordered(eng, shapes, datas, right0, rank_tol, from_host, to_ho
         s, d, r = shapes[i], datas[i], out[i]
         stream = eng.use_slot(i)
         with torch.cuda.stream(stream) if stream is not None else _null():
-            W, b, rec = settle_ls(eng, phase1[i][0], d["feats"], d["b2"], r.idxs, s.k * s.k, r.info["mode"],
+            W, b, rec = settle_ls(eng, phase1[i][0], d["feats"], d["b2"], r.idxs, s.k2, r.info["mode"],
                                   int(chk[0][0]), float(chk[1][0]))
             if W is not None:
                 r.W, r.b = _maybe_to_host(eng, i, W, b, to_host)
@@ -373,14 +385,14 @@ def prune_network_sharded(eng: Engine, shapes, make_data, rank, world_size, righ
     mine = [i for i, o in enumerate(owner) if o == rank]
     datas = [make_data(i) for i in mine]
     res = prune_layers(eng, [shapes[i] for i in mine], datas, right0=right0, rank_tol=rank_tol)
-    sizes = [slot_size(s.c, s.n, s.k * s.k, s.rank, rank_tol) for s in shapes]
+    sizes = [slot_size(s.c, s.n, s.k2, s.rank, rank_tol) for s in shapes]
     # static layout: rank r's buffer holds its problems in index order; pad to the largest rank buffer
     per_rank = [sum(sizes[i] for i in range(len(shapes)) if owner[i] == r) for r in range(world_size)]
     buf = torch.zeros(max(per_rank), dtype=torch.float64, device=eng.device)
     off = 0
     for j, i in enumerate(mine):
         s = shapes[i]
-        pack_result(buf, off, res[j].idxs, res[j].W, res[j].b, res[j].alpha, res[j].nprobe, s.c, s.n, s.k * s.k,
+        pack_result(buf, off, res[j].idxs, res[j].W, res[j].b, res[j].alpha, res[j].nprobe, s.c, s.n, s.k2,
                     eng=eng, slot=j)
         off += sizes[i]
     if world_size > 1:
@@ -395,6 +407,6 @@ def unpack_network(shapes, owner, sizes, allbuf):
     out = [None] * len(shapes)
     for i, s in enumerate(shapes):
         r = owner[i]
-        out[i] = unpack_result(allbuf[r], offs[r], s.c, s.n, s.k * s.k)
+        out[i] = unpack_result(allbuf[r], offs[r], s.c, s.n, s.k2)
         offs[r] += sizes[i]
     return out

@@ -17,6 +17,8 @@ from __future__ import annotations
 
 import numpy as np
 
+from .engine import conv_pair
+
 # (name, c_in, n_out, H=W of the layer's input/output map)  -- temp/vgg.prototxt:53-306
 VGG16 = [
     ("conv1_1", 3, 64, 224), ("conv1_2", 64, 64, 224),
@@ -61,9 +63,20 @@ RESNET50 = [
 
 
 class LayerShape:
-    def __init__(self, name, c, n, H, k=3, pad=1, stride=1, N=5000, B=10, P=10, rank=None):
-        self.name, self.c, self.n, self.H, self.W = name, c, n, H, H
-        self.k, self.pad, self.stride = k, pad, stride
+    """One layer problem: a convolution with c input and n output channels on an H x W input map (W = H unless
+    given).  k, pad, stride and dilation are ints or (h, w) pairs, as torch.nn.Conv2d takes them (groups == 1); the
+    reference's layers are square, odd and undilated, and for those k, pad and stride keep their plain int meaning.
+    kh, kw, pad_h, pad_w, stride_h, stride_w, dil_h, dil_w: the per-axis geometry; k2 = kh*kw taps per channel;
+    Ho x Wo: the output map (PyTorch's formula), the range of the sampled points."""
+
+    def __init__(self, name, c, n, H, k=3, pad=1, stride=1, N=5000, B=10, P=10, rank=None, dilation=1, W=None):
+        self.name, self.c, self.n, self.H, self.W = name, c, n, H, H if W is None else W
+        self.k, self.pad, self.stride, self.dilation = k, pad, stride, dilation
+        self.kh, self.kw = conv_pair(k)
+        self.pad_h, self.pad_w = conv_pair(pad)
+        self.stride_h, self.stride_w = conv_pair(stride)
+        self.dil_h, self.dil_w = conv_pair(dilation)
+        self.k2 = self.kh * self.kw
         self.B, self.P = B, P
         assert N % (B * P) == 0, "N must be a multiple of B*P"
         self.nbatch = N // (B * P)
@@ -71,13 +84,20 @@ class LayerShape:
         self.rank = int(c / C_RATIO) if rank is None else rank
         if c <= 3:
             self.rank = c
-        self.K = c * k * k
+        self.K = c * self.k2
         self.S = min(400, N // 20)
-        self.Ho = (H + 2 * pad - k) // stride + 1  # output map side
+        # output map (torch.nn.Conv2d): (H + 2 pad - dil (k - 1) - 1) // stride + 1 per axis
+        self.Ho = (self.H + 2 * self.pad_h - self.dil_h * (self.kh - 1) - 1) // self.stride_h + 1
+        self.Wo = (self.W + 2 * self.pad_w - self.dil_w * (self.kw - 1) - 1) // self.stride_w + 1
+        assert self.Ho >= 1 and self.Wo >= 1, "empty output map"
+
+    def conv_args(self):
+        """(k, pad, stride) and dilation as Engine.patch_gather takes them"""
+        return dict(k=self.k, pad=self.pad, stride=self.stride, dilation=self.dilation)
 
     def cost(self):
         """Rough relative cost (Gram + Cholesky flops) for load balancing across GPUs."""
-        kp = self.rank * self.k * self.k
+        kp = self.rank * self.k2
         return self.N * self.K * (self.K + 2 * self.n) + kp ** 3 / 3 + 2.0 * kp * kp * self.n
 
 
@@ -93,15 +113,15 @@ def resnet50_layers(N=5000, B=10, P=10):
 def make_problem_numpy(shape: LayerShape, seed: int, noise=0.01):
     """Host (numpy) instance of a layer problem -- used by CPU tests and by the oracle leg.
     Returns dict(fmap (nbatch*B,c,H,W) f32, randx/randy (nbatch,P) i32, W2, b2, feats (N,n) f32,
-    samples (S,), X (N,c,k,k) f32 relu'd patches)."""
+    samples (S,), X (N,c,kh,kw) f32 relu'd patches)."""
     r = np.random.RandomState(seed)
     s = shape
     fmap = r.standard_normal((s.nbatch * s.B, s.c, s.H, s.W)).astype(np.float32)
     randx = r.randint(0, s.Ho, (s.nbatch, s.P)).astype(np.int32)
-    randy = r.randint(0, s.Ho, (s.nbatch, s.P)).astype(np.int32)
-    W2 = (r.standard_normal((s.n, s.c, s.k, s.k)) * np.sqrt(2.0 / (s.c * s.k * s.k))).astype(np.float32)
+    randy = r.randint(0, s.Wo, (s.nbatch, s.P)).astype(np.int32)
+    W2 = (r.standard_normal((s.n, s.c, s.kh, s.kw)) * np.sqrt(2.0 / (s.c * s.k2))).astype(np.float32)
     b2 = (0.01 * r.standard_normal(s.n)).astype(np.float32)
-    X = gather_patches_numpy(fmap, randx, randy, s.B, s.k, s.pad, s.stride, relu=True)
+    X = gather_patches_numpy(fmap, randx, randy, s.B, s.k, s.pad, s.stride, relu=True, dilation=s.dilation)
     Y = X.reshape(s.N, -1).astype(np.float64) @ W2.reshape(s.n, -1).T.astype(np.float64) + b2
     Y = Y + noise * Y.std() * r.standard_normal(Y.shape)
     feats = Y.astype(np.float32)
@@ -109,20 +129,24 @@ def make_problem_numpy(shape: LayerShape, seed: int, noise=0.01):
     return dict(fmap=fmap, randx=randx, randy=randy, W2=W2, b2=b2, feats=feats, samples=samples, X=X)
 
 
-def gather_patches_numpy(fmap, randx, randy, B, k, pad, stride, relu):
+def gather_patches_numpy(fmap, randx, randy, B, k, pad, stride, relu, dilation=1):
     """Plain numpy statement of the patch layout (rows (batch, point, image); columns (c,kh,kw))
     used to build synthetic targets.  (The *checked* restatement of the reference's
-    extract_XY lives in the oracle directory; tests compare the two.)"""
+    extract_XY lives in the oracle directory; tests compare the two.)  k, pad, stride, dilation: ints or (h, w)
+    pairs, as LayerShape takes them."""
+    (kh, kw), (ph, pw), (sh, sw), (dh, dw) = (conv_pair(v) for v in (k, pad, stride, dilation))
     nimg, c, H, W = fmap.shape
     nbatch, P = randx.shape
-    fp = np.zeros((nimg, c, H + 2 * pad, W + 2 * pad), dtype=fmap.dtype)
-    fp[:, :, pad:H + pad, pad:W + pad] = fmap
-    out = np.empty((nbatch * P * B, c, k, k), dtype=fmap.dtype)
+    # taps reach down to stride*(Ho-1) - pad + dil*(k-1) <= H - 1 + pad: a border of pad on each side suffices
+    fp = np.zeros((nimg, c, H + 2 * ph, W + 2 * pw), dtype=fmap.dtype)
+    fp[:, :, ph:H + ph, pw:W + pw] = fmap
+    out = np.empty((nbatch * P * B, c, kh, kw), dtype=fmap.dtype)
     for b in range(nbatch):
         imgs = fp[b * B:(b + 1) * B]
         for p in range(P):
-            y0, x0 = stride * randx[b, p], stride * randy[b, p]
-            out[(b * P + p) * B:(b * P + p + 1) * B] = imgs[:, :, y0:y0 + k, x0:x0 + k]
+            y0, x0 = sh * randx[b, p], sw * randy[b, p]
+            out[(b * P + p) * B:(b * P + p + 1) * B] = imgs[:, :, y0:y0 + dh * (kh - 1) + 1:dh,
+                                                            x0:x0 + dw * (kw - 1) + 1:dw]
     if relu:
         np.maximum(out, 0, out=out)
     return out
@@ -157,11 +181,11 @@ def make_problem_device(shape: LayerShape, seed: int, eng, noise=0.01, pinned_ho
         fmap = fmap.to(dtype)
     r = np.random.RandomState(seed)
     randx = torch.as_tensor(r.randint(0, s.Ho, (s.nbatch, s.P)).astype(np.int32), device=dev)
-    randy = torch.as_tensor(r.randint(0, s.Ho, (s.nbatch, s.P)).astype(np.int32), device=dev)
-    W2 = torch.randn((s.n, s.c, s.k, s.k), generator=g, device=dev, dtype=torch.float32) * float(
-        np.sqrt(2.0 / (s.c * s.k * s.k)))
+    randy = torch.as_tensor(r.randint(0, s.Wo, (s.nbatch, s.P)).astype(np.int32), device=dev)
+    W2 = torch.randn((s.n, s.c, s.kh, s.kw), generator=g, device=dev, dtype=torch.float32) * float(
+        np.sqrt(2.0 / (s.c * s.k2)))
     b2 = 0.01 * torch.randn((s.n,), generator=g, device=dev, dtype=torch.float32)
-    X = eng.patch_gather(fmap, randx, randy, s.B, s.P, s.k, s.pad, s.stride, relu=True)
+    X = eng.patch_gather(fmap, randx, randy, s.B, s.P, relu=True, **s.conv_args())
     Y = X.to(torch.float64) @ W2.reshape(s.n, -1).T.to(torch.float64) + b2.to(torch.float64)
     Y = Y + noise * Y.std() * torch.randn(Y.shape, generator=g, device=dev, dtype=torch.float64)
     feats = Y.to(torch.float32)

@@ -110,6 +110,8 @@ int cp_gram_kernel_ms(cp_handle_t h, float *ms);
  *            blob, zero outside (net.py:564-589, 631-632).
  *   X_out  : (nbatch*P*B) x (c*k*k) fp32, leading dimension ldx (elements),
  *            column = a*k*k + py*k + px.
+ * cp_patch_gather and cp_patch_gather_typed take the reference's square, odd, undilated window (lib/net.py:534-684;
+ * an even k returns CP_ERR_INVALID) and are cp_patch_gather_conv with kh = kw = k, one pad, one stride, dilation 1.
  */
 int cp_patch_gather(cp_handle_t h, const float *fmap, int nbatch, int B, int c, int H, int W, int layout,
                     const int32_t *randx, const int32_t *randy, int P, int k, int pad, int stride, int relu,
@@ -117,6 +119,25 @@ int cp_patch_gather(cp_handle_t h, const float *fmap, int nbatch, int B, int c, 
 int cp_patch_gather_typed(cp_handle_t h, const void *fmap, int fmap_dtype, int nbatch, int B, int c, int H, int W,
                           int layout, const int32_t *randx, const int32_t *randy, int P, int k, int pad, int stride,
                           int relu, float *X_out, int64_t ldx, cp_stream_t stream);
+/*
+ * Patch gather for any torch.nn.Conv2d with groups == 1: rectangular kernels, per-axis padding and stride, dilation.
+ * Output point (x, y) reads the taps
+ *     (stride_h*x - pad_h + dil_h*i, stride_w*y - pad_w + dil_w*j),  i < kh, j < kw,
+ * zero outside the map, into column a*kh*kw + i*kw + j (the order of F.unfold and of W.reshape(n, -1)).  Only the
+ * top / left padding enters the window origin; the bottom / right padding only sets the output size, which the
+ * sampled points already respect -- so padding='same' with an even kernel is one pad per axis too.  The other
+ * arguments are those of cp_patch_gather_typed; ldx >= c*kh*kw.  kh, kw, stride < 1, dilation < 1 or pad < 0 return
+ * CP_ERR_INVALID before any device work.
+ * Paths, as for the square window: NHWC in device memory takes the TMA kernel when its 16-byte rules hold, both
+ * dilations are <= 8, both window spans (k-1)*dil+1 are <= 256 and kh, kw <= 16; other NHWC device maps take the
+ * SIMT kernel (kh*kw <= 95: its shared-memory tile); NHWC maps in pinned host memory take the in-place reader
+ * (kh*kw <= 81); NCHW maps take the SIMT kernel with any window.  A window beyond a path's bound returns
+ * CP_ERR_INVALID.  Square, odd, undilated windows give the bits of cp_patch_gather_typed.
+ */
+int cp_patch_gather_conv(cp_handle_t h, const void *fmap, int fmap_dtype, int nbatch, int B, int c, int H, int W,
+                         int layout, const int32_t *randx, const int32_t *randy, int P, int kh, int kw, int pad_h,
+                         int pad_w, int stride_h, int stride_w, int dil_h, int dil_w, int relu, float *X_out,
+                         int64_t ldx, cp_stream_t stream);
 
 /*
  * Point gather -- replaces the gather of Net.extract_features (lib/net.py:509-519):
