@@ -23,3 +23,10 @@ static inline int cp_fmap_esize(int fmap_dtype) {
 struct cp_window {
     int kh, kw, pad_h, pad_w, stride_h, stride_w, dil_h, dil_w;
 };
+
+// Window of a 3-D patch gather (torch.nn.Conv3d, groups == 1): output point (t, x, y) reads the taps
+// (stride_t*t - pad_t + dil_t*u, stride_h*x - pad_h + dil_h*i, stride_w*y - pad_w + dil_w*j), u < kt, i < kh, j < kw,
+// zero outside the map, into column a*kt*kh*kw + (u*kh + i)*kw + j (the order of Conv3d.weight.reshape(n, -1)).
+struct cp_window3 {
+    int kt, kh, kw, pad_t, pad_h, pad_w, stride_t, stride_h, stride_w, dil_t, dil_h, dil_w;
+};

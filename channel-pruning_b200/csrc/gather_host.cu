@@ -14,6 +14,8 @@
 // Maps whose channel stride or base address is not a multiple of 16 bytes (c = 3, 5, 12 in fp32; odd c in 16 bit)
 // take plain element loads into the same stages: correct for every c, not tuned.
 // The output is bit for bit that of the HBM NHWC kernels: zero outside the map, cp_widen, then fmaxf for the ReLU.
+// NDHWC maps (Conv3d windows, cp_patch_gather_conv3d) take the same pipeline with kt*kh*kw taps per unit: each (u, i)
+// row of an undilated window is again one contiguous run of kw*c elements.
 #include "common.cuh"
 #include "fmap_types.cuh"
 
@@ -30,6 +32,14 @@ struct NhwcHostGeom {
     int tap;      // bytes per tap in a stage: ct * esize + NHWC_HOST_PAD
     int stage;    // bytes per stage
     int vec;      // 16-byte copies (c * esize % 16 == 0, 16-byte aligned map)
+};
+
+// The 3-D form (NDHWC map, Conv3d window); randt rides in the geometry so the pipeline takes the same arguments
+struct NdhwcHostGeom {
+    const int32_t *randt;
+    int B, P, c, D, H, W;
+    cp_window3 w;
+    int ct, nchunk, tap, stage, vec;  // as in NhwcHostGeom
 };
 
 __device__ __forceinline__ void nh_cp_async16(void *smem, const void *gmem) {
@@ -96,12 +106,76 @@ __device__ __forceinline__ void nhwc_host_store(const int32_t *__restrict__ rand
     }
 }
 
-// NS stages: unit u + i * gridDim.x is copied into stage (it + i) % NS while unit u is stored.
-template <int NS, typename T>
-__global__ void __launch_bounds__(256)
-patch_gather_nhwc_host(const T *__restrict__ fmap, const int32_t *__restrict__ randx,
-                       const int32_t *__restrict__ randy, float *__restrict__ X, int64_t ldx, int64_t units,
-                       NhwcHostGeom g, int relu) {
+// Tap p of a 3-D window: (u, i, j) = (p / (kh kw), p / kw % kh, p % kw); its element offset in the image and whether
+// it lies inside the map
+__device__ __forceinline__ bool ndhwc_tap(const NdhwcHostGeom &g, int p, int t0, int y0, int x0, int64_t &off) {
+    const int khw = g.w.kh * g.w.kw;
+    const int pu = p / khw, q = p - pu * khw;
+    const int py = q / g.w.kw, px = q - py * g.w.kw;
+    const int tt = t0 + pu * g.w.dil_t, yy = y0 + py * g.w.dil_h, xx = x0 + px * g.w.dil_w;
+    off = (((int64_t)tt * g.H + yy) * g.W + xx) * g.c;
+    return tt >= 0 && tt < g.D && yy >= 0 && yy < g.H && xx >= 0 && xx < g.W;
+}
+
+template <typename T>
+__device__ __forceinline__ void nhwc_host_fetch(const T *__restrict__ fmap, const int32_t *__restrict__ randx,
+                                                const int32_t *__restrict__ randy, const NdhwcHostGeom &g, int64_t u,
+                                                unsigned char *stage) {
+    const int64_t r = u / g.nchunk;
+    const int a0 = (int)(u - r * g.nchunk) * g.ct;
+    const int ct = min(g.ct, g.c - a0);
+    const int k3 = g.w.kt * g.w.kh * g.w.kw;
+    const int64_t bp = r / g.B;
+    const int img = (int)(bp / g.P) * g.B + (int)(r % g.B);
+    const int t0 = g.w.stride_t * g.randt[bp] - g.w.pad_t;
+    const int y0 = g.w.stride_h * randx[bp] - g.w.pad_h;
+    const int x0 = g.w.stride_w * randy[bp] - g.w.pad_w;
+    const T *src = fmap + (int64_t)img * g.D * g.H * g.W * g.c + a0;
+    int64_t off;
+    if (g.vec) {
+        constexpr int VE = 16 / sizeof(T);
+        const int nv = ct / VE;
+        for (int e = threadIdx.x; e < k3 * nv; e += blockDim.x) {
+            const int p = e / nv, j = e - p * nv;
+            if (ndhwc_tap(g, p, t0, y0, x0, off)) nh_cp_async16(stage + p * g.tap + j * 16, src + off + j * VE);
+        }
+    } else {
+        for (int e = threadIdx.x; e < k3 * ct; e += blockDim.x) {
+            const int p = e / ct, a = e - p * ct;
+            if (ndhwc_tap(g, p, t0, y0, x0, off)) reinterpret_cast<T *>(stage + p * g.tap)[a] = __ldg(src + off + a);
+        }
+    }
+}
+
+template <typename T>
+__device__ __forceinline__ void nhwc_host_store(const int32_t *__restrict__ randx, const int32_t *__restrict__ randy,
+                                                float *__restrict__ X, int64_t ldx, const NdhwcHostGeom &g, int64_t u,
+                                                const unsigned char *stage, int relu) {
+    const int64_t r = u / g.nchunk;
+    const int a0 = (int)(u - r * g.nchunk) * g.ct;
+    const int ct = min(g.ct, g.c - a0);
+    const int k3 = g.w.kt * g.w.kh * g.w.kw;
+    const int64_t bp = r / g.B;
+    const int t0 = g.w.stride_t * g.randt[bp] - g.w.pad_t;
+    const int y0 = g.w.stride_h * randx[bp] - g.w.pad_h;
+    const int x0 = g.w.stride_w * randy[bp] - g.w.pad_w;
+    float *dst = X + r * ldx + (int64_t)a0 * k3;
+    int64_t off;
+    for (int e = threadIdx.x; e < k3 * ct; e += blockDim.x) {
+        const int a = e / k3, p = e - a * k3;
+        float v = 0.f;
+        if (ndhwc_tap(g, p, t0, y0, x0, off)) v = cp_widen(reinterpret_cast<const T *>(stage + p * g.tap)[a]);
+        if (relu) v = fmaxf(v, 0.f);
+        dst[e] = v;
+    }
+}
+
+// NS stages: unit u + i * gridDim.x is copied into stage (it + i) % NS while unit u is stored.  G: NhwcHostGeom or
+// NdhwcHostGeom (the fetch and store of that geometry).
+template <int NS, typename T, typename G>
+__device__ __forceinline__ void host_reader_body(const T *__restrict__ fmap, const int32_t *__restrict__ randx,
+                                                 const int32_t *__restrict__ randy, float *__restrict__ X, int64_t ldx,
+                                                 int64_t units, const G &g, int relu) {
     extern __shared__ __align__(16) unsigned char nh_smem[];
     const int64_t step = gridDim.x;
 #pragma unroll
@@ -123,14 +197,29 @@ patch_gather_nhwc_host(const T *__restrict__ fmap, const int32_t *__restrict__ r
     asm volatile("cp.async.wait_group 0;" ::: "memory");
 }
 
+template <int NS, typename T>
+__global__ void __launch_bounds__(256)
+patch_gather_nhwc_host(const T *__restrict__ fmap, const int32_t *__restrict__ randx,
+                       const int32_t *__restrict__ randy, float *__restrict__ X, int64_t ldx, int64_t units,
+                       NhwcHostGeom g, int relu) {
+    host_reader_body<NS>(fmap, randx, randy, X, ldx, units, g, relu);
+}
+
+template <int NS, typename T>
+__global__ void __launch_bounds__(256)
+patch_gather_ndhwc_host(const T *__restrict__ fmap, const int32_t *__restrict__ randx,
+                        const int32_t *__restrict__ randy, float *__restrict__ X, int64_t ldx, int64_t units,
+                        NdhwcHostGeom g, int relu) {
+    host_reader_body<NS>(fmap, randx, randy, X, ldx, units, g, relu);
+}
+
 }  // namespace
 
-// Geometry of the reader for one map: channel chunk and stage sizes for NS stages.  Returns false when one copy per
-// tap does not fit a stage (never for the kh*kw <= 81 that cp_patch_gather_conv lets through).
-static bool nhwc_host_geom(NhwcHostGeom &g, const void *fmap, int esize, int B, int P, int c, int H, int W,
-                           const cp_window &w, int ns) {
-    const int k2 = w.kh * w.kw;
-    g.B = B, g.P = P, g.c = c, g.H = H, g.W = W, g.w = w;
+// Channel chunk and stage sizes of the reader for a window of k2 taps and NS stages (G: NhwcHostGeom or
+// NdhwcHostGeom).  Returns false when one copy per tap does not fit a stage (never for the kh*kw <= 81 that
+// cp_patch_gather_conv, or the kt*kh*kw <= 343 that cp_patch_gather_conv3d, lets through).
+template <typename G>
+static bool host_chunks(G &g, const void *fmap, int esize, int c, int k2, int ns) {
     g.vec = (c * esize) % 16 == 0 && ((uintptr_t)fmap & 15) == 0;
     const int ve = g.vec ? 16 / esize : 1;
     int ctmax = (NHWC_HOST_SMEM / ns / k2 - NHWC_HOST_PAD) / esize;
@@ -142,6 +231,12 @@ static bool nhwc_host_geom(NhwcHostGeom &g, const void *fmap, int esize, int B, 
     g.tap = g.ct * esize + NHWC_HOST_PAD;
     g.stage = k2 * g.tap;
     return true;
+}
+
+static bool nhwc_host_geom(NhwcHostGeom &g, const void *fmap, int esize, int B, int P, int c, int H, int W,
+                           const cp_window &w, int ns) {
+    g.B = B, g.P = P, g.c = c, g.H = H, g.W = W, g.w = w;
+    return host_chunks(g, fmap, esize, c, w.kh * w.kw, ns);
 }
 
 template <int NS, typename T>
@@ -176,6 +271,29 @@ int cp_patch_gather_nhwc_host(const void *fmap, int fmap_dtype, int nbatch, int 
     else
         launch_nhwc_host<CP_HOST_NHWC_STAGES>((const __half *)fmap, g, rows, randx, randy, relu, X_out, ldx,
                                               CP_HOST_NHWC_GATHER_CTAS, stream);
+    CP_CHECK_LAUNCH();
+    return CP_OK;
+}
+
+int cp_patch_gather_ndhwc_host(const void *fmap, int fmap_dtype, int nbatch, int B, int c, int D, int H, int W,
+                               const int32_t *randt, const int32_t *randx, const int32_t *randy, int P,
+                               const cp_window3 &w, int relu, float *X_out, int64_t ldx, cudaStream_t stream) {
+    NdhwcHostGeom g;
+    g.randt = randt, g.B = B, g.P = P, g.c = c, g.D = D, g.H = H, g.W = W, g.w = w;
+    CP_REQUIRE(host_chunks(g, fmap, cp_fmap_esize(fmap_dtype), c, w.kt * w.kh * w.kw, CP_HOST_NHWC_STAGES),
+               "cp_patch_gather_conv3d: kernel_size %dx%dx%d too large for the NDHWC host reader", w.kt, w.kh, w.kw);
+    const int64_t units = (int64_t)nbatch * P * B * g.nchunk;
+    const unsigned grid = (unsigned)(units < CP_HOST_NHWC_GATHER_CTAS ? units : CP_HOST_NHWC_GATHER_CTAS);
+    const size_t smem = (size_t)CP_HOST_NHWC_STAGES * g.stage;
+    if (fmap_dtype == CP_F32)
+        patch_gather_ndhwc_host<CP_HOST_NHWC_STAGES><<<grid, 256, smem, stream>>>((const float *)fmap, randx, randy,
+                                                                                   X_out, ldx, units, g, relu);
+    else if (fmap_dtype == CP_BF16)
+        patch_gather_ndhwc_host<CP_HOST_NHWC_STAGES><<<grid, 256, smem, stream>>>(
+            (const __nv_bfloat16 *)fmap, randx, randy, X_out, ldx, units, g, relu);
+    else
+        patch_gather_ndhwc_host<CP_HOST_NHWC_STAGES><<<grid, 256, smem, stream>>>((const __half *)fmap, randx, randy,
+                                                                                   X_out, ldx, units, g, relu);
     CP_CHECK_LAUNCH();
     return CP_OK;
 }

@@ -19,6 +19,11 @@
 // bf16 / fp16 maps (template parameter T): the tensor map has the 16-bit data type, the window stage holds 16-bit
 // elements (half the bytes), and the consumers widen exactly while transposing; the row stays fp32.  6 N K bytes.
 // The 16-byte rules of TMA (global strides, box rows) then need c % 8 == 0.
+// NDHWC maps (Conv3d windows, cp_patch_gather_conv3d) take the same kernel body over a 5-D tensor map (c, W, H, D,
+// image): box (c_box, (kw-1)*dil_w+1, (kh-1)*dil_h+1, (kt-1)*dil_t+1, 1), traversal strides (1, dil_w, dil_h, dil_t, 1),
+// one cp.async.bulk.tensor.5d request per box delivering kt x kh x kw taps per channel.  A 3 x 3 x 3 window is three
+// times a 3 x 3 one, so there a work unit is one channel box of a row rather than the whole row: the stage and the
+// output segment (c_box kt kh kw contiguous floats of X) keep the size of the 2-D conv4_x rows.
 #include <cuda.h>
 
 #include "common.cuh"
@@ -36,6 +41,10 @@ struct GtParams {
     int64_t ldx, rows;
     int B, P, c, k2, pad_h, pad_w, stride_h, stride_w, relu, cbox, nbox, nstage;
     int box_f, stage_f, out_f;  // strides in map elements (box, stage) and floats (out); 128-byte multiples each
+    // 5-D maps only: a unit is one channel group of a row -- rows counts units (rows of X x ngrp), c the channels of a
+    // unit (one box), and unit u writes columns [(u % ngrp) c k2, +c k2) of row u / ngrp
+    const int32_t *randt;
+    int stride_t, pad_t, ngrp;
 };
 
 __device__ __forceinline__ uint32_t g_smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -67,14 +76,21 @@ __device__ __forceinline__ void g_tma_load_4d(uint32_t dst, const CUtensorMap *m
         ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
         : "memory");
 }
+__device__ __forceinline__ void g_tma_load_5d(uint32_t dst, const CUtensorMap *map, uint32_t bar, int c0, int c1, int c2, int c3,
+                                              int c4) {
+    asm volatile(
+        "cp.async.bulk.tensor.5d.shared::cta.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
+        ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
+        : "memory");
+}
 __device__ __forceinline__ void g_bulk_store(void *gdst, uint32_t ssrc, uint32_t bytes) {
     asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(ssrc), "r"(bytes) : "memory");
 }
 __device__ __forceinline__ void g_cons_barrier() { asm volatile("bar.sync 1, %0;" ::"n"(GT_CONS) : "memory"); }
 
-template <typename T, int K2>  // map element type; kh*kw known at compile time (1, 9, 25) or 0
-__global__ void __launch_bounds__(GT_THREADS)
-patch_gather_nhwc_tma(const __grid_constant__ CUtensorMap map, const GtParams P) {
+// ND: 4 (NHWC map, whole rows) or 5 (NDHWC map, units of one channel box)
+template <typename T, int K2, int ND>
+__device__ __forceinline__ void gt_body(const CUtensorMap &map, const GtParams &P) {
     extern __shared__ __align__(128) unsigned char gsm_raw[];
     const int k2 = K2 > 0 ? K2 : P.k2, K = P.c * k2;
     const uint32_t stage_bytes = (uint32_t)K * (uint32_t)sizeof(T), row_bytes = (uint32_t)K * 4u;
@@ -102,14 +118,20 @@ patch_gather_nhwc_tma(const __grid_constant__ CUtensorMap map, const GtParams P)
         int it = 0;
         for (int64_t rb = first; rb < P.rows; rb += 32 * step) {
             // lane l looks up the window of row rb + l * step
-            const int64_t r = rb + (int64_t)lane * step;
-            int x0 = 0, y0 = 0, img = 0;
-            if (r < P.rows) {
+            const int64_t u = rb + (int64_t)lane * step;
+            int x0 = 0, y0 = 0, img = 0, t0 = 0, ch0 = 0;
+            if (u < P.rows) {
+                int64_t r = u;
+                if constexpr (ND == 5) {
+                    r = u / P.ngrp;
+                    ch0 = (int)(u - r * P.ngrp) * P.c;
+                }
                 const int img_in_batch = (int)(r % P.B);
                 const int64_t bp = r / P.B;  // batch * P + point
                 const int batch = (int)(bp / P.P);
                 y0 = P.stride_h * P.randx[bp] - P.pad_h;  // window origin, rows  (feat[:,:,x,y]: x indexes H)
                 x0 = P.stride_w * P.randy[bp] - P.pad_w;
+                if constexpr (ND == 5) t0 = P.stride_t * P.randt[bp] - P.pad_t;
                 img = batch * P.B + img_in_batch;
             }
             const int64_t left = (P.rows - rb + step - 1) / step;
@@ -117,15 +139,24 @@ patch_gather_nhwc_tma(const __grid_constant__ CUtensorMap map, const GtParams P)
             for (int j = 0; j < nb; ++j, ++it) {
                 const int xs = __shfl_sync(0xffffffffu, x0, j), ys = __shfl_sync(0xffffffffu, y0, j);
                 const int is = __shfl_sync(0xffffffffu, img, j);
+                int ts = 0, cs = 0;
+                if constexpr (ND == 5) {
+                    ts = __shfl_sync(0xffffffffu, t0, j);
+                    cs = __shfl_sync(0xffffffffu, ch0, j);
+                }
                 if (lane == 0) {
                     const int s = it % P.nstage;
                     const uint32_t ph = (uint32_t)((it / P.nstage) & 1);
                     if (it >= P.nstage) g_mbar_wait(empty(s), ph ^ 1);  // the consumers have released the stage
                     g_mbar_expect_tx(full(s), stage_bytes);
                     const uint32_t dst = g_smem_u32(in + (size_t)s * P.stage_f);
-                    for (int b = 0; b < P.nbox; ++b)
-                        g_tma_load_4d(dst + (uint32_t)b * (uint32_t)P.box_f * (uint32_t)sizeof(T), &map, full(s),
-                                      b * P.cbox, xs, ys, is);
+                    for (int b = 0; b < P.nbox; ++b) {
+                        const uint32_t db = dst + (uint32_t)b * (uint32_t)P.box_f * (uint32_t)sizeof(T);
+                        if constexpr (ND == 5)
+                            g_tma_load_5d(db, &map, full(s), cs + b * P.cbox, xs, ys, ts, is);
+                        else
+                            g_tma_load_4d(db, &map, full(s), b * P.cbox, xs, ys, is);
+                    }
                 }
                 __syncwarp();
             }
@@ -147,11 +178,16 @@ patch_gather_nhwc_tma(const __grid_constant__ CUtensorMap map, const GtParams P)
             const T *sp = src + (size_t)b * P.box_f + al;
             float *dp = dst + (size_t)a * k2;
             if (K2 > 0) {
-                float v[K2 > 0 ? K2 : 1];
+                // loads of a slab batched ahead of its stores; a 3 x 3 x 3 window goes by 3 x 3 slabs (registers)
+                constexpr int KS = K2 > 9 && K2 % 9 == 0 ? 9 : (K2 > 0 ? K2 : 1);
 #pragma unroll
-                for (int p = 0; p < K2; ++p) v[p] = cp_widen(sp[p * P.cbox]);
+                for (int p0 = 0; p0 < K2; p0 += KS) {
+                    float v[KS];
 #pragma unroll
-                for (int p = 0; p < K2; ++p) dp[p] = P.relu ? fmaxf(v[p], 0.f) : v[p];
+                    for (int p = 0; p < KS; ++p) v[p] = cp_widen(sp[(p0 + p) * P.cbox]);
+#pragma unroll
+                    for (int p = 0; p < KS; ++p) dp[p0 + p] = P.relu ? fmaxf(v[p], 0.f) : v[p];
+                }
             } else {
                 for (int p = 0; p < k2; ++p) {
                     float v = cp_widen(sp[(size_t)p * P.cbox]);
@@ -164,20 +200,37 @@ patch_gather_nhwc_tma(const __grid_constant__ CUtensorMap map, const GtParams P)
         g_cons_barrier();
         if (tid == 0) {
             g_mbar_arrive(empty(s));  // every consumer has finished reading in[s]
-            g_bulk_store(P.X + r * P.ldx, g_smem_u32(dst), row_bytes);
+            float *xr = P.X + r * P.ldx;
+            if constexpr (ND == 5) {
+                const int64_t row = r / P.ngrp;
+                xr = P.X + row * P.ldx + (r - row * P.ngrp) * (int64_t)K;
+            }
+            g_bulk_store(xr, g_smem_u32(dst), row_bytes);
             asm volatile("cp.async.bulk.commit_group;" ::: "memory");
         }
     }
     if (tid == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // shared memory must outlive the reads
 }
 
+template <typename T, int K2>  // map element type; kh*kw known at compile time (1, 9, 25) or 0
+__global__ void __launch_bounds__(GT_THREADS)
+patch_gather_nhwc_tma(const __grid_constant__ CUtensorMap map, const GtParams P) {
+    gt_body<T, K2, 4>(map, P);
+}
+
+template <typename T, int K2>  // map element type; kt*kh*kw known at compile time (1, 9, 27) or 0
+__global__ void __launch_bounds__(GT_THREADS)
+patch_gather_ndhwc_tma(const __grid_constant__ CUtensorMap map, const GtParams P) {
+    gt_body<T, K2, 5>(map, P);
+}
+
 inline size_t gt_round128(size_t b) { return (b + 127) & ~(size_t)127; }
 
 // Elements one tiled TMA request delivers to shared memory: ceil(boxDim[i] / elementStrides[i]) per dimension (the
 // rule of the cuTensorMapEncodeTiled documentation)
-inline size_t gt_box_elems(const cuuint32_t box[4], const cuuint32_t estr[4]) {
+inline size_t gt_box_elems(const cuuint32_t *box, const cuuint32_t *estr, int rank) {
     size_t n = 1;
-    for (int i = 0; i < 4; ++i) n *= (box[i] + estr[i] - 1) / estr[i];
+    for (int i = 0; i < rank; ++i) n *= (box[i] + estr[i] - 1) / estr[i];
     return n;
 }
 
@@ -186,6 +239,21 @@ typedef CUresult (*encode_fn_t)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, 
                                 CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
 }  // namespace
+
+typedef void (*gt_kernel_t)(const CUtensorMap, const GtParams);
+
+static int gt_run(cp_handle_t h, gt_kernel_t kern, cp_per_device_flag &configured, const CUtensorMap &map,
+                  const GtParams &Pm, size_t smem, int per_sm, cudaStream_t stream) {
+    if (bool *done = configured.slot(); !*done) {
+        CP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+        *done = true;
+    }
+    int64_t grid = (int64_t)h->num_sms * per_sm;
+    if (grid > Pm.rows) grid = Pm.rows;
+    kern<<<(unsigned)grid, GT_THREADS, smem, stream>>>(map, Pm);
+    CP_CHECK_LAUNCH();
+    return CP_OK;
+}
 
 template <typename T>
 static int gt_launch(cp_handle_t h, const CUtensorMap &map, const GtParams &Pm, size_t smem, int per_sm,
@@ -196,15 +264,48 @@ static int gt_launch(cp_handle_t h, const CUtensorMap &map, const GtParams &Pm, 
               : k2 == 25 ? patch_gather_nhwc_tma<T, 25> : patch_gather_nhwc_tma<T, 0>;
     static cp_per_device_flag configured[4];  // one set per element type (one per instantiation of gt_launch)
     const int which = k2 == 9 ? 0 : k2 == 1 ? 1 : k2 == 25 ? 2 : 3;
-    if (bool *done = configured[which].slot(); !*done) {
-        CP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-        *done = true;
+    return gt_run(h, kern, configured[which], map, Pm, smem, per_sm, stream);
+}
+
+template <typename T>
+static int gt_launch3d(cp_handle_t h, const CUtensorMap &map, const GtParams &Pm, size_t smem, int per_sm,
+                       cudaStream_t stream) {
+    // 3 x 3 x 3, 1 x 3 x 3 (the spatial half of R(2+1)D) and 1 x 1 x 1 at compile time
+    const int k2 = Pm.k2;
+    auto kern = k2 == 27 ? patch_gather_ndhwc_tma<T, 27> : k2 == 9 ? patch_gather_ndhwc_tma<T, 9>
+              : k2 == 1 ? patch_gather_ndhwc_tma<T, 1> : patch_gather_ndhwc_tma<T, 0>;
+    static cp_per_device_flag configured[4];
+    const int which = k2 == 27 ? 0 : k2 == 9 ? 1 : k2 == 1 ? 2 : 3;
+    return gt_run(h, kern, configured[which], map, Pm, smem, per_sm, stream);
+}
+
+// CTAs per SM and input stages for a window stage of `row` bytes and output rows of `out_b` bytes: as many CTAs as fit
+// with >= 2 input stages each (up to 4), then the stages fill what is left.
+// conv4_x (c = 512, k = 3): fp32 stage 18 KB, row 18 KB -> 2 CTAs x 3 stages; 16-bit stage 9 KB, row 18 KB ->
+// 3 CTAs x 3 stages (the fp32 output rows then take most of the budget)
+static void gt_ring(size_t row, size_t out_b, int &per_sm, int &nstage) {
+    const size_t budget = 216 * 1024;
+    per_sm = (int)(budget / (2 * row + GT_OUT * out_b + 1024));
+    per_sm = per_sm < 1 ? 1 : (per_sm > 4 ? 4 : per_sm);
+    nstage = (int)((budget / per_sm - 1024 - GT_OUT * out_b) / row);
+    if (nstage > 6) nstage = 6;
+}
+
+static int gt_encode_fn(cp_handle_t h) {
+    if (!h->tmap_encode) {
+        void *fn = nullptr;
+        cudaDriverEntryPointQueryResult qres;
+        CP_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
+        if (!fn || qres != cudaDriverEntryPointSuccess) CP_FAIL(CP_ERR_CUDA, "cuTensorMapEncodeTiled not available");
+        h->tmap_encode = fn;
     }
-    int64_t grid = (int64_t)h->num_sms * per_sm;
-    if (grid > Pm.rows) grid = Pm.rows;
-    kern<<<(unsigned)grid, GT_THREADS, smem, stream>>>(map, Pm);
-    CP_CHECK_LAUNCH();
     return CP_OK;
+}
+
+static CUtensorMapDataType gt_dtype(int fmap_dtype) {
+    return fmap_dtype == CP_BF16  ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+           : fmap_dtype == CP_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
+                                  : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
 }
 
 // Channels per TMA box: the largest divisor of c in [16, 256] whose box row is a multiple of 16 bytes (TMA), 0 if none
@@ -241,13 +342,7 @@ bool cp_gather_tma_eligible(const void *fmap, int esize, int c, const cp_window 
 int cp_patch_gather_tma(cp_handle_t h, const void *fmap, int fmap_dtype, int nbatch, int B, int c, int H, int W,
                         const int32_t *randx, const int32_t *randy, int P, const cp_window &g, int relu,
                         float *X_out, int64_t ldx, cudaStream_t stream) {
-    if (!h->tmap_encode) {
-        void *fn = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        CP_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
-        if (!fn || qres != cudaDriverEntryPointSuccess) CP_FAIL(CP_ERR_CUDA, "cuTensorMapEncodeTiled not available");
-        h->tmap_encode = fn;
-    }
+    if (int rc = gt_encode_fn(h)) return rc;
     const int esize = cp_fmap_esize(fmap_dtype);
     const int cbox = gt_cbox(c, esize);
     const int64_t nimg = (int64_t)nbatch * B;
@@ -258,10 +353,7 @@ int cp_patch_gather_tma(cp_handle_t h, const void *fmap, int fmap_dtype, int nba
     const cuuint32_t box[4] = {(cuuint32_t)cbox, (cuuint32_t)((g.kw - 1) * g.dil_w + 1),
                                (cuuint32_t)((g.kh - 1) * g.dil_h + 1), 1};
     const cuuint32_t estr[4] = {1, (cuuint32_t)g.dil_w, (cuuint32_t)g.dil_h, 1};
-    const CUtensorMapDataType dt = fmap_dtype == CP_BF16  ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
-                                   : fmap_dtype == CP_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
-                                                          : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
-    CUresult cr = ((encode_fn_t)h->tmap_encode)(&map, dt, 4, (void *)fmap, dims, strides, box, estr,
+    CUresult cr = ((encode_fn_t)h->tmap_encode)(&map, gt_dtype(fmap_dtype), 4, (void *)fmap, dims, strides, box, estr,
                                                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
                                                 CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (cr != CUDA_SUCCESS) CP_FAIL(CP_ERR_CUDA, "cuTensorMapEncodeTiled (4-D feature map) failed (%d)", (int)cr);
@@ -274,23 +366,97 @@ int cp_patch_gather_tma(cp_handle_t h, const void *fmap, int fmap_dtype, int nba
     Pm.cbox = cbox; Pm.nbox = c / cbox;
     // Bytes the copy engine delivers per box, hence what expect_tx must announce (the kernel arms c * k2 * esize per
     // window): ceil(box[i] / estr[i]) elements per dimension, i.e. cbox x kw x kh x 1 (gt_box_elems).
-    const size_t box_b = gt_round128(gt_box_elems(box, estr) * esize), row = box_b * Pm.nbox;
-    if (gt_box_elems(box, estr) != (size_t)cbox * k2)
+    const size_t box_b = gt_round128(gt_box_elems(box, estr, 4) * esize), row = box_b * Pm.nbox;
+    if (gt_box_elems(box, estr, 4) != (size_t)cbox * k2)
         CP_FAIL(CP_ERR_CUDA, "cp_patch_gather: TMA box delivers %zu elements, the window has %zu",
-                gt_box_elems(box, estr), (size_t)cbox * k2);
+                gt_box_elems(box, estr, 4), (size_t)cbox * k2);
     const size_t out_b = gt_round128((size_t)c * k2 * 4);
-    // CTAs per SM: as many as fit with >= 2 input stages each (up to 4), then the stages fill what is left.
-    // conv4_x (c = 512, k = 3): fp32 stage 18 KB, row 18 KB -> 2 CTAs x 3 stages; 16-bit stage 9 KB, row 18 KB ->
-    // 3 CTAs x 3 stages (the fp32 output rows then take most of the budget)
-    const size_t budget = 216 * 1024;
-    int per_sm = (int)(budget / (2 * row + GT_OUT * out_b + 1024));
-    per_sm = per_sm < 1 ? 1 : (per_sm > 4 ? 4 : per_sm);
-    int nstage = (int)((budget / per_sm - 1024 - GT_OUT * out_b) / row);
-    if (nstage > 6) nstage = 6;
+    int per_sm, nstage;
+    gt_ring(row, out_b, per_sm, nstage);
     Pm.nstage = nstage;
     Pm.box_f = (int)(box_b / esize); Pm.stage_f = (int)(row / esize); Pm.out_f = (int)(out_b / 4);
     const size_t smem = (size_t)nstage * row + GT_OUT * out_b + 2 * nstage * 8 + 256;
     if (fmap_dtype == CP_BF16) return gt_launch<__nv_bfloat16>(h, map, Pm, smem, per_sm, stream);
     if (fmap_dtype == CP_F16) return gt_launch<__half>(h, map, Pm, smem, per_sm, stream);
     return gt_launch<float>(h, map, Pm, smem, per_sm, stream);
+}
+
+// ---------------------------------------------------------------------------------------------------- 5-D (NDHWC)
+
+// Bytes of one work unit's output segment the 3-D path aims at: the fp32 row of the 2-D path at conv4_x (c = 512,
+// 3 x 3), which that path moves at its best rate.  A 3 x 3 x 3 window at c >= 128 is split into 128-channel units.
+constexpr size_t GT3_UNIT_BYTES = 18 * 1024;
+
+// Channels per box (= per work unit) of the 3-D path: the largest divisor of c in [16, 256] with whole 16-byte box rows
+// whose fp32 output segment is at most GT3_UNIT_BYTES; the smallest such divisor when none is; 0 when c has none
+static int gt_cbox3d(int c, int esize, int k3) {
+    int last = 0;
+    for (int d = 256; d >= 16; d -= 16 / esize) {
+        if (c % d) continue;
+        if ((size_t)d * k3 * 4 <= GT3_UNIT_BYTES) return d;
+        last = d;
+    }
+    return last;
+}
+
+bool cp_gather_tma3d_eligible(const void *fmap, int esize, int c, const cp_window3 &g, float *X_out, int64_t ldx) {
+    if (c % (16 / esize) || c < 16 || g.kt > 16 || g.kh > 16 || g.kw > 16) return false;
+    if (g.dil_t > GT_MAX_DIL || g.dil_h > GT_MAX_DIL || g.dil_w > GT_MAX_DIL) return false;
+    if ((g.kt - 1) * g.dil_t + 1 > GT_MAX_SPAN || (g.kh - 1) * g.dil_h + 1 > GT_MAX_SPAN ||
+        (g.kw - 1) * g.dil_w + 1 > GT_MAX_SPAN)
+        return false;
+    if (((uintptr_t)fmap & 15) || ((uintptr_t)X_out & 15) || (ldx % 4)) return false;
+    cudaPointerAttributes pa;
+    if (cudaPointerGetAttributes(&pa, fmap) != cudaSuccess || pa.type != cudaMemoryTypeDevice) {
+        (void)cudaGetLastError();
+        return false;
+    }
+    const int k3 = g.kt * g.kh * g.kw;
+    const int cbox = gt_cbox3d(c, esize, k3);
+    if (!cbox) return false;
+    const size_t row = gt_round128((size_t)cbox * k3 * esize), out_b = gt_round128((size_t)cbox * k3 * 4);
+    return 2 * row + GT_OUT * (row > out_b ? row : out_b) + 1024 <= 200 * 1024;
+}
+
+int cp_patch_gather_tma3d(cp_handle_t h, const void *fmap, int fmap_dtype, int nbatch, int B, int c, int D, int H,
+                          int W, const int32_t *randt, const int32_t *randx, const int32_t *randy, int P,
+                          const cp_window3 &g, int relu, float *X_out, int64_t ldx, cudaStream_t stream) {
+    if (int rc = gt_encode_fn(h)) return rc;
+    const int esize = cp_fmap_esize(fmap_dtype);
+    const int k3 = g.kt * g.kh * g.kw;
+    const int cbox = gt_cbox3d(c, esize, k3);
+    const int64_t nimg = (int64_t)nbatch * B;
+    CUtensorMap map;
+    const cuuint64_t dims[5] = {(cuuint64_t)c, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)D, (cuuint64_t)nimg};
+    const cuuint64_t pix = (cuuint64_t)c * esize;
+    const cuuint64_t strides[4] = {pix, W * pix, (cuuint64_t)H * W * pix, (cuuint64_t)D * H * W * pix};
+    // the box spans the dilated window; the traversal strides pick its kw x kh x kt taps, which land densely
+    const cuuint32_t box[5] = {(cuuint32_t)cbox, (cuuint32_t)((g.kw - 1) * g.dil_w + 1),
+                               (cuuint32_t)((g.kh - 1) * g.dil_h + 1), (cuuint32_t)((g.kt - 1) * g.dil_t + 1), 1};
+    const cuuint32_t estr[5] = {1, (cuuint32_t)g.dil_w, (cuuint32_t)g.dil_h, (cuuint32_t)g.dil_t, 1};
+    CUresult cr = ((encode_fn_t)h->tmap_encode)(&map, gt_dtype(fmap_dtype), 5, (void *)fmap, dims, strides, box, estr,
+                                                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+                                                CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (cr != CUDA_SUCCESS) CP_FAIL(CP_ERR_CUDA, "cuTensorMapEncodeTiled (5-D feature map) failed (%d)", (int)cr);
+    // expect_tx announces cbox * kt * kh * kw elements per unit: what the copy engine delivers by the ceil rule
+    if (gt_box_elems(box, estr, 5) != (size_t)cbox * k3)
+        CP_FAIL(CP_ERR_CUDA, "cp_patch_gather_conv3d: TMA box delivers %zu elements, the window has %zu",
+                gt_box_elems(box, estr, 5), (size_t)cbox * k3);
+    GtParams Pm{};
+    Pm.randx = randx; Pm.randy = randy; Pm.randt = randt; Pm.X = X_out; Pm.ldx = ldx;
+    Pm.ngrp = c / cbox;
+    Pm.rows = (int64_t)nbatch * P * B * Pm.ngrp;  // work units
+    Pm.B = B; Pm.P = P; Pm.c = cbox; Pm.k2 = k3; Pm.relu = relu;
+    Pm.pad_t = g.pad_t; Pm.pad_h = g.pad_h; Pm.pad_w = g.pad_w;
+    Pm.stride_t = g.stride_t; Pm.stride_h = g.stride_h; Pm.stride_w = g.stride_w;
+    Pm.cbox = cbox; Pm.nbox = 1;
+    const size_t row = gt_round128((size_t)cbox * k3 * esize), out_b = gt_round128((size_t)cbox * k3 * 4);
+    int per_sm, nstage;
+    gt_ring(row, out_b, per_sm, nstage);
+    Pm.nstage = nstage;
+    Pm.box_f = (int)(row / esize); Pm.stage_f = Pm.box_f; Pm.out_f = (int)(out_b / 4);
+    const size_t smem = (size_t)nstage * row + GT_OUT * out_b + 2 * nstage * 8 + 256;
+    if (fmap_dtype == CP_BF16) return gt_launch3d<__nv_bfloat16>(h, map, Pm, smem, per_sm, stream);
+    if (fmap_dtype == CP_F16) return gt_launch3d<__half>(h, map, Pm, smem, per_sm, stream);
+    return gt_launch3d<float>(h, map, Pm, smem, per_sm, stream);
 }

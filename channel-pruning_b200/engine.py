@@ -30,6 +30,7 @@ MAX_PROBES = 64
 LS_RATIO_MIN = 0.005
 
 _LAYOUTS = {"nchw": 0, "nhwc": 1}
+_LAYOUTS3D = {"ncdhw": 0, "ndhwc": 1}  # the same C codes, with a depth axis
 GRAM_FP64, GRAM_3XTF32 = 0, 1
 # element types of the feature maps the gathers read (CP_F32, CP_BF16, CP_F16 of include/cpb200.h)
 FMAP_DTYPES = {torch.float32: 0, torch.bfloat16: 2, torch.float16: 3}
@@ -41,6 +42,14 @@ def conv_pair(v):
         assert len(v) == 2, v
         return int(v[0]), int(v[1])
     return int(v), int(v)
+
+
+def conv_triple(v):
+    """(t, h, w) of a Conv3d-style argument given as an int or a triple (kernel_size, padding, stride, dilation)."""
+    if isinstance(v, (tuple, list)):
+        assert len(v) == 3, v
+        return int(v[0]), int(v[1]), int(v[2])
+    return int(v), int(v), int(v)
 
 
 def fmap_dtype_code(dtype):
@@ -287,6 +296,56 @@ class Engine:
                                                   _LAYOUTS[layout], self._p(randx, "const int32_t*"),
                                                   self._p(randy, "const int32_t*"), P, self._p(out, "float*"),
                                                   out.stride(0), self._s()))
+        return out
+
+    def patch_gather3d(self, fmap, randt, randx, randy, B, P, k, pad, stride, relu=True, layout="ncdhw", out=None,
+                       dilation=1):
+        """fmap: (nbatch*B, c, D, H, W) [ncdhw] or (nbatch*B, D, H, W, c) [ndhwc, channels_last_3d], float32 /
+        bfloat16 / float16, on device or in pinned host memory (read in place); randt/randx/randy: (nbatch, P) int32 on
+        device, the sampled output points (t, x, y).  Returns X (nbatch*P*B, c*kt*kh*kw) fp32, 16-bit maps widened
+        exactly.  k, pad, stride, dilation: an int or a (t, h, w) triple, with the meaning of torch.nn.Conv3d's
+        arguments (pad: the front / top / left padding).  Columns are in Conv3d.weight.reshape(n, -1)'s order."""
+        dt = fmap_dtype_code(fmap.dtype)
+        assert fmap.is_contiguous() and fmap.dim() == 5
+        nimg = fmap.shape[0]
+        assert nimg % B == 0
+        nbatch = nimg // B
+        if layout == "ncdhw":
+            c, D, H, W = fmap.shape[1:]
+        else:
+            D, H, W, c = fmap.shape[1:]
+        for r in (randt, randx, randy):
+            assert r.dtype == torch.int32 and r.numel() == nbatch * P and r.is_contiguous()
+        (kt, kh, kw), (pt, ph, pw), (st, sh, sw), (dt_, dh, dw) = (conv_triple(v) for v in (k, pad, stride, dilation))
+        rows, K = nbatch * P * B, c * kt * kh * kw
+        if out is None:
+            out = self.empty(rows, K, dtype=torch.float32)
+        assert out.shape == (rows, K) and out.dtype == torch.float32 and out.stride(1) == 1
+        self._call(self.lib.cp_patch_gather_conv3d(
+            self.h, self._p(fmap, "const void*"), dt, nbatch, B, c, D, H, W, _LAYOUTS3D[layout],
+            self._p(randt, "const int32_t*"), self._p(randx, "const int32_t*"), self._p(randy, "const int32_t*"), P,
+            kt, kh, kw, pt, ph, pw, st, sh, sw, dt_, dh, dw, int(bool(relu)), self._p(out, "float*"), out.stride(0),
+            self._s()))
+        return out
+
+    def point_gather3d(self, fmap, randt, randx, randy, B, P, layout="ncdhw", out=None):
+        """Y (nbatch*P*B, n) fp32 at the sampled points (t, x, y) of a Conv3d output map (nbatch*B, n, To, Ho, Wo)
+        [ncdhw] or (nbatch*B, To, Ho, Wo, n) [ndhwc], float32 / bfloat16 / float16 widened exactly."""
+        dt = fmap_dtype_code(fmap.dtype)
+        assert fmap.is_contiguous() and fmap.dim() == 5
+        nbatch = fmap.shape[0] // B
+        if layout == "ncdhw":
+            n, D, H, W = fmap.shape[1:]
+        else:
+            D, H, W, n = fmap.shape[1:]
+        rows = nbatch * P * B
+        if out is None:
+            out = self.empty(rows, n, dtype=torch.float32)
+        assert out.shape == (rows, n) and out.dtype == torch.float32 and out.stride(1) == 1
+        self._call(self.lib.cp_point_gather3d(
+            self.h, self._p(fmap, "const void*"), dt, nbatch, B, n, D, H, W, _LAYOUTS3D[layout],
+            self._p(randt, "const int32_t*"), self._p(randx, "const int32_t*"), self._p(randy, "const int32_t*"), P,
+            self._p(out, "float*"), out.stride(0), self._s()))
         return out
 
     def gram(self, X, Y=None, y_bias=None, rows=None, want_G=True, want_B=True, want_sums=True, want_yy=False,

@@ -70,6 +70,7 @@ def dictionary(X, W2, Y, alpha=1e-4, rank=None, DEBUG=0, B2=None, rank_tol=.1, v
     X: (N, c, h, w)   W2: (n, c, h, w)   Y: (N, n)   rank: channels to keep
     returns (idxs bool[c], newW2 (n, c', h, w) float64, newB2 (n,) float64)
     h != w (a 1 x 7 or 3 x 1 layer) is accepted: columns are (c, h, w) in that order, as F.unfold gives them.
+    Conv3d layers: X (N, c, t, h, w), W2 (n, c, t, h, w) -> newW2 (n, c', t, h, w); columns (c, t, h, w).
     or, with DEBUG, (newX, newW2, newB2) (decompose.py:629-632).
 
     Reference behaviour that is kept on purpose:
@@ -87,15 +88,17 @@ def dictionary(X, W2, Y, alpha=1e-4, rank=None, DEBUG=0, B2=None, rank_tol=.1, v
             dcfgs.dic.debug or dcfgs.fc_ridge or dcfgs.nonlinear_fc or dcfgs.nofc:
         raise NotImplementedError("only the `train.py -action c3` configuration of dictionary() is implemented")
     eng = get_engine()
-    N, c, h, w = X.shape[0], X.shape[1], X.shape[2], X.shape[3]
+    N, c, win = X.shape[0], X.shape[1], tuple(int(v) for v in X.shape[2:])  # win: (h, w), or (t, h, w) for Conv3d
+    assert len(win) in (2, 3), "X must be (N, c, h, w) or (N, c, t, h, w)"
+    k2 = int(np.prod(win))
     n = W2.shape[0]
-    assert tuple(X.shape) == (N, c, h, w) and tuple(W2.shape) == (n, c, h, w) and tuple(Y.shape) == (N, n)
-    Xd = _dev_f32(X, eng).reshape(N, c * h * w)
-    W2m = _dev_f32(W2, eng).reshape(n, c * h * w)
+    assert tuple(W2.shape) == (n, c) + win and tuple(Y.shape) == (N, n)
+    Xd = _dev_f32(X, eng).reshape(N, c * k2)
+    W2m = _dev_f32(W2, eng).reshape(n, c * k2)
     Yd = _dev_y(Y, eng)
-    idxs, Wd, bd = _dictionary_device(eng, Xd, W2m, Yd, None, c, h * w, rank, alpha)
+    idxs, Wd, bd = _dictionary_device(eng, Xd, W2m, Yd, None, c, k2, rank, alpha)
     rank = int(idxs.sum())
-    newW2 = Wd.cpu().numpy().reshape((n, rank, h, w))
+    newW2 = Wd.cpu().numpy().reshape((n, rank) + win)
     newB2 = bd.cpu().numpy()
     if DEBUG:
         Xh = X.cpu().numpy() if isinstance(X, torch.Tensor) else np.asarray(X)

@@ -78,13 +78,18 @@ def pack_result(buf, offset, idxs, W, b, alpha, nprobe, c, n, k2, eng=None, slot
     buf[offset + 4 + c + n:offset + 4 + c + n + n * cp * k2] = W.reshape(-1).to(buf.device, torch.float64)
 
 
-def unpack_result(buf, offset, c, n, k2):
+def unpack_result(buf, offset, c, n, k2, window=None):
+    """window: the layer's kernel extents, (kh, kw) or (kt, kh, kw) with product k2 -- W comes back (n, c', *window);
+    None: a square k x k window, k = sqrt(k2)."""
     head = buf[offset:offset + 4].cpu().numpy()
     cp = int(head[0])
     idxs = buf[offset + 4:offset + 4 + c].cpu().numpy() != 0
     b = buf[offset + 4 + c:offset + 4 + c + n].cpu().numpy()
-    k = int(round(np.sqrt(k2)))
-    W = buf[offset + 4 + c + n:offset + 4 + c + n + n * cp * k2].cpu().numpy().reshape(n, cp, k, k)
+    if window is None:
+        k = int(round(np.sqrt(k2)))
+        window = (k, k)
+    assert int(np.prod(window)) == k2, (window, k2)
+    W = buf[offset + 4 + c + n:offset + 4 + c + n + n * cp * k2].cpu().numpy().reshape((n, cp) + tuple(window))
     return dict(idxs=idxs, W=W, b=b, alpha=float(head[1]), nprobe=int(head[2]))
 
 
@@ -107,6 +112,8 @@ def prune_layers(eng: Engine, shapes, datas, right0=1e-3, rank_tol=.1, from_host
     ``eng``.  from_host: feature maps are taken from pinned host memory (datas[i]['fmap_host'], float32, bfloat16
     or float16, laid out as datas[i]['host_layout']: 'nchw' (default) or 'nhwc') and copied in the pipeline; to_host:
     results are copied back to pinned host memory.
+    Conv3d layers (synth.LayerShape3d, whose data carry randt) may stand alone or among 2-D ones; their layouts are
+    'ncdhw' (default) or 'ndhwc'.
     trace: optional dict; filled with {layer name: [(label, timing event), ...]} plus '_t0' (device timeline
     of the step: profiles/e2e_breakdown.py prints it).
     Batch mode: the problems are INDEPENDENT -- every alpha search starts from ``right0`` and the seeds come with the
@@ -141,6 +148,28 @@ ZC_LINES_PER_S = 2.6e8
 ZC_NHWC_LINES_PER_S = 7.1e7
 
 
+def window_of(s):
+    """Kernel extents of a layer shape: (kh, kw), or (kt, kh, kw) for a Conv3d layer (synth.LayerShape3d)."""
+    return (s.kt, s.kh, s.kw) if _is3d(s) else (getattr(s, "kh", s.k), getattr(s, "kw", s.k))
+
+
+def _is3d(s):
+    return hasattr(s, "kt")
+
+
+def _default_layout(s):
+    return "ncdhw" if _is3d(s) else "nchw"
+
+
+def _patch_gather(eng, s, d, fmap, layout):
+    """The gather of layer s from map fmap (layout as the map lies): Engine.patch_gather3d for a Conv3d layer
+    (d carries randt), Engine.patch_gather otherwise."""
+    if _is3d(s):
+        return eng.patch_gather3d(fmap, d["randt"], d["randx"], d["randy"], s.B, s.P, relu=True, layout=layout,
+                                  **s.conv_args())
+    return eng.patch_gather(fmap, d["randx"], d["randy"], s.B, s.P, relu=True, layout=layout, **s.conv_args())
+
+
 def zero_copy_lines(s, esize=4, layout="nchw"):
     """128-byte lines the in-place gather touches in host memory (esize: bytes per map element), for a window of
     kh x kw taps with dilation (dil_h, dil_w) (s.kh, s.kw, s.dilation; a shape with only s.k is square, undilated).
@@ -151,7 +180,12 @@ def zero_copy_lines(s, esize=4, layout="nchw"):
     pixel stride c*esize is not a multiple of 128 bytes (a run may then start inside a line).  An upper bound for a
     map whose base is 128-byte aligned: clipping at the border only removes lines.
     Square, undilated windows give the counts the transfer rates ZC_LINES_PER_S and ZC_NHWC_LINES_PER_S were
-    measured with."""
+    measured with.
+    Conv3d layers (s.kt): 'ncdhw' counts c*kt*kh rows of kw taps, 'ndhwc' kt*kh runs of kw*c*esize bytes -- kt times
+    the 2-D count of the (kh, kw) window rows of one frame (frames are H*W pixels apart)."""
+    if _is3d(s):
+        flat = _Frame(s)
+        return s.kt * zero_copy_lines(flat, esize, "nhwc" if layout in ("nhwc", "ndhwc") else "nchw")
     kh, kw = getattr(s, "kh", s.k), getattr(s, "kw", s.k)
     dh, dw = conv_pair(getattr(s, "dilation", 1))
     span_w = (kw - 1) * dw + 1  # elements from the first tap of a window row to its last
@@ -168,9 +202,17 @@ def zero_copy_lines(s, esize=4, layout="nchw"):
     return s.N * s.c * lines
 
 
+class _Frame:
+    """The (kh, kw) window of a Conv3d layer on one frame: what zero_copy_lines counts per temporal tap."""
+
+    def __init__(self, s):
+        self.N, self.c, self.W, self.kh, self.kw = s.N, s.c, s.W, s.kh, s.kw
+        self.k, self.dilation = s.kh, (s.dil_h, s.dil_w)
+
+
 def _zero_copy_seconds(s, esize=4, layout="nchw"):
     """Model of the in-place gather over PCIe: it is bound by the number of read requests."""
-    rate = ZC_NHWC_LINES_PER_S if layout == "nhwc" else ZC_LINES_PER_S
+    rate = ZC_NHWC_LINES_PER_S if layout in ("nhwc", "ndhwc") else ZC_LINES_PER_S
     return zero_copy_lines(s, esize, layout) / rate
 
 
@@ -197,7 +239,7 @@ def h2d_plan(shapes, datas, from_host):
         esize = _element_size(d["fmap_host"])
         nbytes = d["fmap_host"].numel() * esize
         t_dma = nbytes / 50e9 + 1e-4
-        t_zc = _zero_copy_seconds(s, esize, d.get("host_layout", "nchw"))
+        t_zc = _zero_copy_seconds(s, esize, d.get("host_layout", _default_layout(s)))
         plan.append("dma" if (nbytes <= cap and t_dma < ratio * t_zc) else "zc")
     return plan
 
@@ -234,8 +276,7 @@ def _prune_layers_ordered(eng, shapes, datas, right0, rank_tol, from_host, to_ho
                 continue
             eng.use_slot(i)
             with torch.cuda.stream(zc_stream):
-                X = eng.patch_gather(d["fmap_host"], d["randx"], d["randy"], s.B, s.P, relu=True,
-                                     layout=d.get("host_layout", "nchw"), **s.conv_args())
+                X = _patch_gather(eng, s, d, d["fmap_host"], d.get("host_layout", _default_layout(s)))
                 _mark(trace, s.name, "zc_done")
                 ev = torch.cuda.Event()
                 ev.record()
@@ -248,7 +289,7 @@ def _prune_layers_ordered(eng, shapes, datas, right0, rank_tol, from_host, to_ho
             if stream is not None:
                 stream.wait_stream(main)
             X = None
-            layout = d.get("host_layout", "nchw")  # of fmap_host, and of its staged copy in HBM
+            layout = d.get("host_layout", _default_layout(s))  # of fmap_host, and of its staged copy in HBM
             if pre[i] is not None:
                 kind, obj, ev = pre[i]
                 stream.wait_event(ev)
@@ -265,10 +306,9 @@ def _prune_layers_ordered(eng, shapes, datas, right0, rank_tol, from_host, to_ho
                 fmap = d["fmap_host"]
             else:
                 fmap = d["fmap"]
-                layout = d.get("layout", "nchw")  # HBM layout of fmap
+                layout = d.get("layout", _default_layout(s))  # HBM layout of fmap
             if X is None:
-                X = eng.patch_gather(fmap, d["randx"], d["randy"], s.B, s.P, relu=True, layout=layout,
-                                     **s.conv_args())
+                X = _patch_gather(eng, s, d, fmap, layout)
             W2m = d["W2"].reshape(s.n, s.K)
             if s.rank == s.c:
                 g_full = eng.gram(X, d["feats"], y_bias=d["b2"])
@@ -407,6 +447,6 @@ def unpack_network(shapes, owner, sizes, allbuf):
     out = [None] * len(shapes)
     for i, s in enumerate(shapes):
         r = owner[i]
-        out[i] = unpack_result(allbuf[r], offs[r], s.c, s.n, s.k2)
+        out[i] = unpack_result(allbuf[r], offs[r], s.c, s.n, s.k2, window_of(s))
         offs[r] += sizes[i]
     return out

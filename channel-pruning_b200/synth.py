@@ -17,7 +17,7 @@ from __future__ import annotations
 
 import numpy as np
 
-from .engine import conv_pair
+from .engine import conv_pair, conv_triple
 
 # (name, c_in, n_out, H=W of the layer's input/output map)  -- temp/vgg.prototxt:53-306
 VGG16 = [
@@ -101,6 +101,67 @@ class LayerShape:
         return self.N * self.K * (self.K + 2 * self.n) + kp ** 3 / 3 + 2.0 * kp * kp * self.n
 
 
+class LayerShape3d:
+    """One layer problem of a Conv3d consumer with c input and n output channels on a D x H x W input map (W = H unless
+    given).  k, pad, stride and dilation are ints or (t, h, w) triples, as torch.nn.Conv3d takes them (groups == 1).
+    kt, kh, kw, pad_t, ..., dil_w: the per-axis geometry; k2 = kt*kh*kw taps per channel (what the solver sees: X is
+    (N, c*k2)); To x Ho x Wo: the output map (PyTorch's formula), the range of the sampled points (t, x, y)."""
+
+    def __init__(self, name, c, n, D, H, k=3, pad=1, stride=1, N=5000, B=10, P=10, rank=None, dilation=1, W=None):
+        self.name, self.c, self.n, self.D, self.H, self.W = name, c, n, D, H, H if W is None else W
+        self.k, self.pad, self.stride, self.dilation = k, pad, stride, dilation
+        self.kt, self.kh, self.kw = conv_triple(k)
+        self.pad_t, self.pad_h, self.pad_w = conv_triple(pad)
+        self.stride_t, self.stride_h, self.stride_w = conv_triple(stride)
+        self.dil_t, self.dil_h, self.dil_w = conv_triple(dilation)
+        self.window = (self.kt, self.kh, self.kw)
+        self.k2 = self.kt * self.kh * self.kw
+        self.B, self.P = B, P
+        assert N % (B * P) == 0, "N must be a multiple of B*P"
+        self.nbatch = N // (B * P)
+        self.N = N
+        self.rank = int(c / C_RATIO) if rank is None else rank
+        if c <= 3:
+            self.rank = c
+        self.K = c * self.k2
+        self.S = min(400, N // 20)
+        # output map (torch.nn.Conv3d): (in + 2 pad - dil (k - 1) - 1) // stride + 1 per axis
+        self.To = (self.D + 2 * self.pad_t - self.dil_t * (self.kt - 1) - 1) // self.stride_t + 1
+        self.Ho = (self.H + 2 * self.pad_h - self.dil_h * (self.kh - 1) - 1) // self.stride_h + 1
+        self.Wo = (self.W + 2 * self.pad_w - self.dil_w * (self.kw - 1) - 1) // self.stride_w + 1
+        assert self.To >= 1 and self.Ho >= 1 and self.Wo >= 1, "empty output map"
+
+    def conv_args(self):
+        """(k, pad, stride) and dilation as Engine.patch_gather3d takes them"""
+        return dict(k=self.k, pad=self.pad, stride=self.stride, dilation=self.dilation)
+
+    def cost(self):
+        """Rough relative cost (Gram + Cholesky flops) for load balancing across GPUs."""
+        kp = self.rank * self.k2
+        return self.N * self.K * (self.K + 2 * self.n) + kp ** 3 / 3 + 2.0 * kp * kp * self.n
+
+
+# torchvision's r3d_18 on a 16 x 112 x 112 clip: the 3x3x3 convolutions of layer1-layer4 (two BasicBlocks each).
+# (name, c_in, n_out, D = H of the layer's INPUT map, stride); the first conv of layer2-4 halves every axis.
+R3D18 = [
+    ("layer1.0.conv1", 64, 64, 16, 56, 1), ("layer1.0.conv2", 64, 64, 16, 56, 1),
+    ("layer1.1.conv1", 64, 64, 16, 56, 1), ("layer1.1.conv2", 64, 64, 16, 56, 1),
+    ("layer2.0.conv1", 64, 128, 16, 56, 2), ("layer2.0.conv2", 128, 128, 8, 28, 1),
+    ("layer2.1.conv1", 128, 128, 8, 28, 1), ("layer2.1.conv2", 128, 128, 8, 28, 1),
+    ("layer3.0.conv1", 128, 256, 8, 28, 2), ("layer3.0.conv2", 256, 256, 4, 14, 1),
+    ("layer3.1.conv1", 256, 256, 4, 14, 1), ("layer3.1.conv2", 256, 256, 4, 14, 1),
+    ("layer4.0.conv1", 256, 512, 4, 14, 2), ("layer4.0.conv2", 512, 512, 2, 7, 1),
+    ("layer4.1.conv1", 512, 512, 2, 7, 1), ("layer4.1.conv2", 512, 512, 2, 7, 1),
+]
+
+
+def r3d18_layers(N=5000, B=10, P=50):
+    """The 16 layer problems of R3D18.  B = 10 clips and P = 50 points per batch (10 batches at N = 5000) keep the
+    synthetic fp32 maps at 8.1 GB in all (6.4 GB of them the five 64 x 16 x 56 x 56 maps); with P = 10 they would be
+    50 batches, 40 GB."""
+    return [LayerShape3d(nm, c, n, D, H, k=3, pad=1, stride=st, N=N, B=B, P=P) for nm, c, n, D, H, st in R3D18]
+
+
 def vgg16_layers(N=5000, B=10, P=10):
     return [LayerShape(nm, c, n, H, N=N, B=B, P=P) for nm, c, n, H in VGG16]
 
@@ -114,6 +175,8 @@ def make_problem_numpy(shape: LayerShape, seed: int, noise=0.01):
     """Host (numpy) instance of a layer problem -- used by CPU tests and by the oracle leg.
     Returns dict(fmap (nbatch*B,c,H,W) f32, randx/randy (nbatch,P) i32, W2, b2, feats (N,n) f32,
     samples (S,), X (N,c,kh,kw) f32 relu'd patches)."""
+    if isinstance(shape, LayerShape3d):
+        return _make_problem3d_numpy(shape, seed, noise)
     r = np.random.RandomState(seed)
     s = shape
     fmap = r.standard_normal((s.nbatch * s.B, s.c, s.H, s.W)).astype(np.float32)
@@ -152,6 +215,43 @@ def gather_patches_numpy(fmap, randx, randy, B, k, pad, stride, relu, dilation=1
     return out
 
 
+def _make_problem3d_numpy(s, seed, noise):
+    """make_problem_numpy for a LayerShape3d: fmap (nbatch*B, c, D, H, W), randt/randx/randy, X (N, c, kt, kh, kw)."""
+    r = np.random.RandomState(seed)
+    fmap = r.standard_normal((s.nbatch * s.B, s.c, s.D, s.H, s.W)).astype(np.float32)
+    randt = r.randint(0, s.To, (s.nbatch, s.P)).astype(np.int32)
+    randx = r.randint(0, s.Ho, (s.nbatch, s.P)).astype(np.int32)
+    randy = r.randint(0, s.Wo, (s.nbatch, s.P)).astype(np.int32)
+    W2 = (r.standard_normal((s.n, s.c) + s.window) * np.sqrt(2.0 / (s.c * s.k2))).astype(np.float32)
+    b2 = (0.01 * r.standard_normal(s.n)).astype(np.float32)
+    X = gather_patches3d_numpy(fmap, randt, randx, randy, s.B, s.k, s.pad, s.stride, relu=True, dilation=s.dilation)
+    Y = X.reshape(s.N, -1).astype(np.float64) @ W2.reshape(s.n, -1).T.astype(np.float64) + b2
+    Y = Y + noise * Y.std() * r.standard_normal(Y.shape)
+    feats = Y.astype(np.float32)
+    samples = r.randint(0, s.N, s.S)
+    return dict(fmap=fmap, randt=randt, randx=randx, randy=randy, W2=W2, b2=b2, feats=feats, samples=samples, X=X)
+
+
+def gather_patches3d_numpy(fmap, randt, randx, randy, B, k, pad, stride, relu, dilation=1):
+    """gather_patches_numpy for NCDHW maps and Conv3d windows: rows (batch, point, image), columns (c, kt, kh, kw).
+    k, pad, stride, dilation: ints or (t, h, w) triples."""
+    (kt, kh, kw), (pt, ph, pw), (st, sh, sw), (dt, dh, dw) = (conv_triple(v) for v in (k, pad, stride, dilation))
+    nimg, c, D, H, W = fmap.shape
+    nbatch, P = randx.shape
+    fp = np.zeros((nimg, c, D + 2 * pt, H + 2 * ph, W + 2 * pw), dtype=fmap.dtype)
+    fp[:, :, pt:D + pt, ph:H + ph, pw:W + pw] = fmap
+    out = np.empty((nbatch * P * B, c, kt, kh, kw), dtype=fmap.dtype)
+    for b in range(nbatch):
+        imgs = fp[b * B:(b + 1) * B]
+        for p in range(P):
+            t0, y0, x0 = st * randt[b, p], sh * randx[b, p], sw * randy[b, p]
+            out[(b * P + p) * B:(b * P + p + 1) * B] = imgs[:, :, t0:t0 + dt * (kt - 1) + 1:dt,
+                                                            y0:y0 + dh * (kh - 1) + 1:dh, x0:x0 + dw * (kw - 1) + 1:dw]
+    if relu:
+        np.maximum(out, 0, out=out)
+    return out
+
+
 def fmap_nchw(d):
     """The feature map of a problem dict in the reference's blob order (nimg, c, H, W), whatever its HBM layout."""
     return d["fmap"].permute(0, 3, 1, 2) if d.get("layout", "nchw") == "nhwc" else d["fmap"]
@@ -172,6 +272,8 @@ def make_problem_device(shape: LayerShape, seed: int, eng, noise=0.01, pinned_ho
     targets are computed from the rounded map."""
     import torch
 
+    if isinstance(shape, LayerShape3d):
+        return _make_problem3d_device(shape, seed, eng, noise, pinned_host, layout, dtype, host_layout)
     s = shape
     dev = eng.device
     g = torch.Generator(device=dev)
@@ -205,5 +307,43 @@ def make_problem_device(shape: LayerShape, seed: int, eng, noise=0.01, pinned_ho
         out["fmap_host"].copy_(fmap)
     if layout == "nhwc":
         out["fmap"] = fmap.permute(0, 2, 3, 1).contiguous()
+        del fmap
+    return out
+
+
+def _make_problem3d_device(s, seed, eng, noise, pinned_host, layout, dtype, host_layout):
+    """make_problem_device for a LayerShape3d.  layout / host_layout: 'ncdhw' or 'ndhwc' ('nchw' / 'nhwc', the 2-D
+    defaults, are read as their 3-D forms); the dict carries both keys and randt."""
+    import torch
+
+    layout = {"nchw": "ncdhw", "nhwc": "ndhwc"}.get(layout, layout)
+    host_layout = {"nchw": "ncdhw", "nhwc": "ndhwc"}.get(host_layout, host_layout)
+    assert layout in ("ncdhw", "ndhwc") and host_layout in ("ncdhw", "ndhwc"), (layout, host_layout)
+    dev = eng.device
+    g = torch.Generator(device=dev)
+    g.manual_seed(seed)
+    fmap = torch.randn((s.nbatch * s.B, s.c, s.D, s.H, s.W), generator=g, device=dev, dtype=torch.float32)
+    if dtype is not None and dtype != torch.float32:
+        fmap = fmap.to(dtype)
+    r = np.random.RandomState(seed)
+    pts = [torch.as_tensor(r.randint(0, hi, (s.nbatch, s.P)).astype(np.int32), device=dev) for hi in (s.To, s.Ho, s.Wo)]
+    W2 = torch.randn((s.n, s.c) + s.window, generator=g, device=dev, dtype=torch.float32) * float(
+        np.sqrt(2.0 / (s.c * s.k2)))
+    b2 = 0.01 * torch.randn((s.n,), generator=g, device=dev, dtype=torch.float32)
+    X = eng.patch_gather3d(fmap, *pts, s.B, s.P, relu=True, **s.conv_args())
+    Y = X.to(torch.float64) @ W2.reshape(s.n, -1).T.to(torch.float64) + b2.to(torch.float64)
+    Y = Y + noise * Y.std() * torch.randn(Y.shape, generator=g, device=dev, dtype=torch.float64)
+    feats = Y.to(torch.float32)
+    samples = torch.as_tensor(r.randint(0, s.N, s.S).astype(np.int32), device=dev)
+    seeds = r.randint(0, 2147483647, size=64)
+    out = dict(fmap=fmap, randt=pts[0], randx=pts[1], randy=pts[2], W2=W2, b2=b2, feats=feats, samples=samples,
+               seeds=seeds, layout=layout, host_layout=host_layout)
+    del X, Y
+    if pinned_host:
+        src = fmap.permute(0, 2, 3, 4, 1) if host_layout == "ndhwc" else fmap
+        out["fmap_host"] = torch.empty(src.shape, dtype=fmap.dtype, pin_memory=True)
+        out["fmap_host"].copy_(src)
+    if layout == "ndhwc":
+        out["fmap"] = fmap.permute(0, 2, 3, 4, 1).contiguous()
         del fmap
     return out

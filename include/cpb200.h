@@ -140,6 +140,29 @@ int cp_patch_gather_conv(cp_handle_t h, const void *fmap, int fmap_dtype, int nb
                          int64_t ldx, cp_stream_t stream);
 
 /*
+ * Patch gather for torch.nn.Conv3d (groups == 1): 3-D maps of video and volumetric networks.
+ *   fmap   : nbatch*B images, layout CP_LAYOUT_NCHW meaning NCDHW (B,c,D,H,W) or CP_LAYOUT_NHWC meaning NDHWC
+ *            (B,D,H,W,c, channels_last_3d); fmap_dtype CP_F32 | CP_BF16 | CP_F16, widened exactly; device memory or
+ *            page-locked host memory (read in place), as for the 2-D gathers.
+ *   randt, randx, randy : nbatch*P sampled output points (t, x, y), t < To, x < Ho, y < Wo.
+ * Output point (t, x, y) reads the taps
+ *     (stride_t*t - pad_t + dil_t*u,  stride_h*x - pad_h + dil_h*i,  stride_w*y - pad_w + dil_w*j),
+ * u < kt, i < kh, j < kw, zero outside the map, into column a*kt*kh*kw + (u*kh + i)*kw + j (the order of
+ * Conv3d.weight.reshape(n, -1)); relu as in cp_patch_gather_conv.  X_out: (nbatch*P*B) x (c*kt*kh*kw) fp32, ldx >=
+ * c*kt*kh*kw.  Before any device work, CP_ERR_INVALID for: an extent, stride or dilation < 1, a padding < 0, more
+ * than 4096 taps, or an empty output map ((in + 2 pad - dil (k - 1) - 1) / stride + 1 < 1 on an axis).
+ * Paths: NDHWC in device memory takes the TMA kernel (5-D tensor map, one request per window and channel box) under
+ * the rules of the 2-D TMA path (16-byte rules, c >= 16, every extent <= 16, dilations <= 8, spans <= 256); NDHWC in
+ * pinned host memory the in-place reader (kt*kh*kw <= 343, else CP_ERR_INVALID); other NDHWC device maps the SIMT
+ * kernel; NCDHW maps the SIMT kernel.  Results are bit-identical across paths.
+ */
+int cp_patch_gather_conv3d(cp_handle_t h, const void *fmap, int fmap_dtype, int nbatch, int B, int c, int D, int H,
+                           int W, int layout, const int32_t *randt, const int32_t *randx, const int32_t *randy, int P,
+                           int kt, int kh, int kw, int pad_t, int pad_h, int pad_w, int stride_t, int stride_h,
+                           int stride_w, int dil_t, int dil_h, int dil_w, int relu, float *X_out, int64_t ldx,
+                           cp_stream_t stream);
+
+/*
  * Point gather -- replaces the gather of Net.extract_features (lib/net.py:509-519):
  *   Y_out[(batch*P+point)*B + image, j] = fmap[batch*B+image, j, randx, randy].
  * fp32 out (the reference widens to fp64; the bias of lib/net.py:1707 is applied
@@ -152,6 +175,12 @@ int cp_point_gather(cp_handle_t h, const float *fmap, int nbatch, int B, int n, 
 int cp_point_gather_typed(cp_handle_t h, const void *fmap, int fmap_dtype, int nbatch, int B, int n, int H, int W,
                           int layout, const int32_t *randx, const int32_t *randy, int P, float *Y_out, int64_t ldy,
                           cp_stream_t stream);
+/* The same for the output map of a Conv3d consumer, (B,n,D,H,W) (CP_LAYOUT_NCHW: NCDHW) or (B,D,H,W,n)
+ * (CP_LAYOUT_NHWC: NDHWC):  Y_out[(batch*P+point)*B + image, j] = fmap[batch*B+image, j, randt, randx, randy].
+ * An empty map (n, D, H or W < 1) returns CP_ERR_INVALID. */
+int cp_point_gather3d(cp_handle_t h, const void *fmap, int fmap_dtype, int nbatch, int B, int n, int D, int H, int W,
+                      int layout, const int32_t *randt, const int32_t *randx, const int32_t *randy, int P,
+                      float *Y_out, int64_t ldy, cp_stream_t stream);
 
 /*
  * Tall-skinny Gram / cross products -- replaces the O(N K^2) arithmetic inside
