@@ -1,5 +1,5 @@
-// In-place reader of channels-last (NHWC) feature maps in pinned host memory: the patch gather of the host-resident
-// input path for maps a channels_last forward hands over (cp_patch_gather_typed, layout NHWC, map in page-locked host
+// In-place reader of channels-last (NHWC / NDHWC) feature maps in pinned host memory: the patch gather of the
+// host-resident input path for maps a channels_last forward hands over (layout CP_LAYOUT_NHWC, map in page-locked host
 // memory mapped under UVA).
 //
 // Over PCIe a gather costs read requests, not bytes.  In NHWC the in-bounds taps of an undilated window row are one
@@ -14,8 +14,8 @@
 // Maps whose channel stride or base address is not a multiple of 16 bytes (c = 3, 5, 12 in fp32; odd c in 16 bit)
 // take plain element loads into the same stages: correct for every c, not tuned.
 // The output is bit for bit that of the HBM NHWC kernels: zero outside the map, cp_widen, then fmaxf for the ReLU.
-// NDHWC maps (Conv3d windows, cp_patch_gather_conv3d) take the same pipeline with kt*kh*kw taps per unit: each (u, i)
-// row of an undilated window is again one contiguous run of kw*c elements.
+// NDHWC maps (Conv3d windows, DEPTH = true) take kt*kh*kw taps per unit: each (u, i) row of an undilated window is
+// again one contiguous run of kw*c elements.
 #include "common.cuh"
 #include "fmap_types.cuh"
 
@@ -24,8 +24,9 @@ namespace {
 constexpr int NHWC_HOST_SMEM = 48 * 1024;  // shared memory of a CTA (all stages)
 constexpr int NHWC_HOST_PAD = 16;          // bytes after each tap of a stage: keeps 16-byte alignment, spreads banks
 
-struct NhwcHostGeom {
-    int B, P, c, H, W;
+struct HostGeom {
+    const int32_t *randt;  // NULL: a 2-D map (D = 1, t = 0)
+    int B, P, c, D, H, W;
     cp_window w;
     int ct;       // channels per chunk (the last chunk may be shorter)
     int nchunk;   // chunks per window
@@ -34,218 +35,140 @@ struct NhwcHostGeom {
     int vec;      // 16-byte copies (c * esize % 16 == 0, 16-byte aligned map)
 };
 
-// The 3-D form (NDHWC map, Conv3d window); randt rides in the geometry so the pipeline takes the same arguments
-struct NdhwcHostGeom {
-    const int32_t *randt;
-    int B, P, c, D, H, W;
-    cp_window3 w;
-    int ct, nchunk, tap, stage, vec;  // as in NhwcHostGeom
-};
-
 __device__ __forceinline__ void nh_cp_async16(void *smem, const void *gmem) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem)),
                  "l"(gmem) : "memory");
 }
 
 // Starts the copy of unit u into `stage`: 16-byte cp.async requests, or (vec == 0) plain element loads.
-template <typename T>
-__device__ __forceinline__ void nhwc_host_fetch(const T *__restrict__ fmap, const int32_t *__restrict__ randx,
-                                                const int32_t *__restrict__ randy, const NhwcHostGeom &g, int64_t u,
-                                                unsigned char *stage) {
+template <bool DEPTH, typename T>
+__device__ __forceinline__ void host_fetch(const T *__restrict__ fmap, const int32_t *__restrict__ randx,
+                                           const int32_t *__restrict__ randy, const HostGeom &g, int64_t u,
+                                           unsigned char *stage) {
     const int64_t r = u / g.nchunk;
     const int a0 = (int)(u - r * g.nchunk) * g.ct;
     const int ct = min(g.ct, g.c - a0);
-    const int k2 = g.w.kh * g.w.kw;
+    const int k = (DEPTH ? g.w.kt : 1) * g.w.kh * g.w.kw;
     const int64_t bp = r / g.B;
     const int img = (int)(bp / g.P) * g.B + (int)(r % g.B);
+    const int t0 = DEPTH ? g.w.stride_t * g.randt[bp] - g.w.pad_t : 0;
     const int y0 = g.w.stride_h * randx[bp] - g.w.pad_h;
     const int x0 = g.w.stride_w * randy[bp] - g.w.pad_w;
-    const T *src = fmap + (int64_t)img * g.H * g.W * g.c + a0;
+    const T *src = fmap + (int64_t)img * (DEPTH ? g.D : 1) * g.H * g.W * g.c + a0;
+    int tt, yy, xx;
     if (g.vec) {
         constexpr int VE = 16 / sizeof(T);  // elements per copy
         const int nv = ct / VE;
-        for (int e = threadIdx.x; e < k2 * nv; e += blockDim.x) {
+        for (int e = threadIdx.x; e < k * nv; e += blockDim.x) {
             const int p = e / nv, j = e - p * nv;
-            const int py = p / g.w.kw, px = p - py * g.w.kw;
-            const int yy = y0 + py * g.w.dil_h, xx = x0 + px * g.w.dil_w;
-            if (yy >= 0 && yy < g.H && xx >= 0 && xx < g.W)
-                nh_cp_async16(stage + p * g.tap + j * 16, src + ((int64_t)yy * g.W + xx) * g.c + j * VE);
+            if (cp_window_tap<DEPTH>(g.w, p, t0, y0, x0, g.D, g.H, g.W, tt, yy, xx))
+                nh_cp_async16(stage + p * g.tap + j * 16, src + cp_pixel<DEPTH>(tt, yy, xx, g.H, g.W) * g.c + j * VE);
         }
     } else {
-        for (int e = threadIdx.x; e < k2 * ct; e += blockDim.x) {
+        for (int e = threadIdx.x; e < k * ct; e += blockDim.x) {
             const int p = e / ct, a = e - p * ct;
-            const int py = p / g.w.kw, px = p - py * g.w.kw;
-            const int yy = y0 + py * g.w.dil_h, xx = x0 + px * g.w.dil_w;
-            if (yy >= 0 && yy < g.H && xx >= 0 && xx < g.W)
-                reinterpret_cast<T *>(stage + p * g.tap)[a] = __ldg(src + ((int64_t)yy * g.W + xx) * g.c + a);
+            if (cp_window_tap<DEPTH>(g.w, p, t0, y0, x0, g.D, g.H, g.W, tt, yy, xx))
+                reinterpret_cast<T *>(stage + p * g.tap)[a] = __ldg(src + cp_pixel<DEPTH>(tt, yy, xx, g.H, g.W) * g.c + a);
         }
     }
 }
 
-// Writes unit u from its stage: column a*kh*kw + p of the chunk, zero for taps outside the map.
-template <typename T>
-__device__ __forceinline__ void nhwc_host_store(const int32_t *__restrict__ randx, const int32_t *__restrict__ randy,
-                                                float *__restrict__ X, int64_t ldx, const NhwcHostGeom &g, int64_t u,
-                                                const unsigned char *stage, int relu) {
+// Writes unit u from its stage: column a*taps + p of the chunk, zero for taps outside the map.
+template <bool DEPTH, typename T>
+__device__ __forceinline__ void host_store(const int32_t *__restrict__ randx, const int32_t *__restrict__ randy,
+                                           float *__restrict__ X, int64_t ldx, const HostGeom &g, int64_t u,
+                                           const unsigned char *stage, int relu) {
     const int64_t r = u / g.nchunk;
     const int a0 = (int)(u - r * g.nchunk) * g.ct;
     const int ct = min(g.ct, g.c - a0);
-    const int k2 = g.w.kh * g.w.kw;
+    const int k = (DEPTH ? g.w.kt : 1) * g.w.kh * g.w.kw;
     const int64_t bp = r / g.B;
+    const int t0 = DEPTH ? g.w.stride_t * g.randt[bp] - g.w.pad_t : 0;
     const int y0 = g.w.stride_h * randx[bp] - g.w.pad_h;
     const int x0 = g.w.stride_w * randy[bp] - g.w.pad_w;
-    float *dst = X + r * ldx + (int64_t)a0 * k2;
-    for (int e = threadIdx.x; e < k2 * ct; e += blockDim.x) {
-        const int a = e / k2, p = e - a * k2;
-        const int py = p / g.w.kw, px = p - py * g.w.kw;
-        const int yy = y0 + py * g.w.dil_h, xx = x0 + px * g.w.dil_w;
+    float *dst = X + r * ldx + (int64_t)a0 * k;
+    int tt, yy, xx;
+    for (int e = threadIdx.x; e < k * ct; e += blockDim.x) {
+        const int a = e / k, p = e - a * k;
         float v = 0.f;
-        if (yy >= 0 && yy < g.H && xx >= 0 && xx < g.W) v = cp_widen(reinterpret_cast<const T *>(stage + p * g.tap)[a]);
+        if (cp_window_tap<DEPTH>(g.w, p, t0, y0, x0, g.D, g.H, g.W, tt, yy, xx))
+            v = cp_widen(reinterpret_cast<const T *>(stage + p * g.tap)[a]);
         if (relu) v = fmaxf(v, 0.f);
         dst[e] = v;
     }
 }
 
-// Tap p of a 3-D window: (u, i, j) = (p / (kh kw), p / kw % kh, p % kw); its element offset in the image and whether
-// it lies inside the map
-__device__ __forceinline__ bool ndhwc_tap(const NdhwcHostGeom &g, int p, int t0, int y0, int x0, int64_t &off) {
-    const int khw = g.w.kh * g.w.kw;
-    const int pu = p / khw, q = p - pu * khw;
-    const int py = q / g.w.kw, px = q - py * g.w.kw;
-    const int tt = t0 + pu * g.w.dil_t, yy = y0 + py * g.w.dil_h, xx = x0 + px * g.w.dil_w;
-    off = (((int64_t)tt * g.H + yy) * g.W + xx) * g.c;
-    return tt >= 0 && tt < g.D && yy >= 0 && yy < g.H && xx >= 0 && xx < g.W;
-}
-
-template <typename T>
-__device__ __forceinline__ void nhwc_host_fetch(const T *__restrict__ fmap, const int32_t *__restrict__ randx,
-                                                const int32_t *__restrict__ randy, const NdhwcHostGeom &g, int64_t u,
-                                                unsigned char *stage) {
-    const int64_t r = u / g.nchunk;
-    const int a0 = (int)(u - r * g.nchunk) * g.ct;
-    const int ct = min(g.ct, g.c - a0);
-    const int k3 = g.w.kt * g.w.kh * g.w.kw;
-    const int64_t bp = r / g.B;
-    const int img = (int)(bp / g.P) * g.B + (int)(r % g.B);
-    const int t0 = g.w.stride_t * g.randt[bp] - g.w.pad_t;
-    const int y0 = g.w.stride_h * randx[bp] - g.w.pad_h;
-    const int x0 = g.w.stride_w * randy[bp] - g.w.pad_w;
-    const T *src = fmap + (int64_t)img * g.D * g.H * g.W * g.c + a0;
-    int64_t off;
-    if (g.vec) {
-        constexpr int VE = 16 / sizeof(T);
-        const int nv = ct / VE;
-        for (int e = threadIdx.x; e < k3 * nv; e += blockDim.x) {
-            const int p = e / nv, j = e - p * nv;
-            if (ndhwc_tap(g, p, t0, y0, x0, off)) nh_cp_async16(stage + p * g.tap + j * 16, src + off + j * VE);
-        }
-    } else {
-        for (int e = threadIdx.x; e < k3 * ct; e += blockDim.x) {
-            const int p = e / ct, a = e - p * ct;
-            if (ndhwc_tap(g, p, t0, y0, x0, off)) reinterpret_cast<T *>(stage + p * g.tap)[a] = __ldg(src + off + a);
-        }
-    }
-}
-
-template <typename T>
-__device__ __forceinline__ void nhwc_host_store(const int32_t *__restrict__ randx, const int32_t *__restrict__ randy,
-                                                float *__restrict__ X, int64_t ldx, const NdhwcHostGeom &g, int64_t u,
-                                                const unsigned char *stage, int relu) {
-    const int64_t r = u / g.nchunk;
-    const int a0 = (int)(u - r * g.nchunk) * g.ct;
-    const int ct = min(g.ct, g.c - a0);
-    const int k3 = g.w.kt * g.w.kh * g.w.kw;
-    const int64_t bp = r / g.B;
-    const int t0 = g.w.stride_t * g.randt[bp] - g.w.pad_t;
-    const int y0 = g.w.stride_h * randx[bp] - g.w.pad_h;
-    const int x0 = g.w.stride_w * randy[bp] - g.w.pad_w;
-    float *dst = X + r * ldx + (int64_t)a0 * k3;
-    int64_t off;
-    for (int e = threadIdx.x; e < k3 * ct; e += blockDim.x) {
-        const int a = e / k3, p = e - a * k3;
-        float v = 0.f;
-        if (ndhwc_tap(g, p, t0, y0, x0, off)) v = cp_widen(reinterpret_cast<const T *>(stage + p * g.tap)[a]);
-        if (relu) v = fmaxf(v, 0.f);
-        dst[e] = v;
-    }
-}
-
-// NS stages: unit u + i * gridDim.x is copied into stage (it + i) % NS while unit u is stored.  G: NhwcHostGeom or
-// NdhwcHostGeom (the fetch and store of that geometry).
-template <int NS, typename T, typename G>
+// NS stages: unit u + i * gridDim.x is copied into stage (it + i) % NS while unit u is stored.
+template <int NS, bool DEPTH, typename T>
 __device__ __forceinline__ void host_reader_body(const T *__restrict__ fmap, const int32_t *__restrict__ randx,
                                                  const int32_t *__restrict__ randy, float *__restrict__ X, int64_t ldx,
-                                                 int64_t units, const G &g, int relu) {
+                                                 int64_t units, const HostGeom &g, int relu) {
     extern __shared__ __align__(16) unsigned char nh_smem[];
     const int64_t step = gridDim.x;
 #pragma unroll
     for (int i = 0; i < NS - 1; ++i) {
         const int64_t ui = blockIdx.x + i * step;
-        if (ui < units) nhwc_host_fetch(fmap, randx, randy, g, ui, nh_smem + i * g.stage);
+        if (ui < units) host_fetch<DEPTH>(fmap, randx, randy, g, ui, nh_smem + i * g.stage);
         asm volatile("cp.async.commit_group;" ::: "memory");
     }
     int it = 0;
     for (int64_t u = blockIdx.x; u < units; u += step, ++it) {
         const int64_t un = u + (NS - 1) * step;
-        if (un < units) nhwc_host_fetch(fmap, randx, randy, g, un, nh_smem + ((it + NS - 1) % NS) * g.stage);
+        if (un < units) host_fetch<DEPTH>(fmap, randx, randy, g, un, nh_smem + ((it + NS - 1) % NS) * g.stage);
         asm volatile("cp.async.commit_group;" ::: "memory");
         asm volatile("cp.async.wait_group %0;" ::"n"(NS - 1) : "memory");  // unit u's copies have landed
         __syncthreads();
-        nhwc_host_store<T>(randx, randy, X, ldx, g, u, nh_smem + (it % NS) * g.stage, relu);
+        host_store<DEPTH, T>(randx, randy, X, ldx, g, u, nh_smem + (it % NS) * g.stage, relu);
         __syncthreads();  // the stage is refilled NS - 1 units later
     }
     asm volatile("cp.async.wait_group 0;" ::: "memory");
 }
 
+// The reader by name, one per rank (profiles and tests tell the paths apart by it)
 template <int NS, typename T>
 __global__ void __launch_bounds__(256)
 patch_gather_nhwc_host(const T *__restrict__ fmap, const int32_t *__restrict__ randx,
                        const int32_t *__restrict__ randy, float *__restrict__ X, int64_t ldx, int64_t units,
-                       NhwcHostGeom g, int relu) {
-    host_reader_body<NS>(fmap, randx, randy, X, ldx, units, g, relu);
+                       HostGeom g, int relu) {
+    host_reader_body<NS, false>(fmap, randx, randy, X, ldx, units, g, relu);
 }
-
 template <int NS, typename T>
 __global__ void __launch_bounds__(256)
 patch_gather_ndhwc_host(const T *__restrict__ fmap, const int32_t *__restrict__ randx,
                         const int32_t *__restrict__ randy, float *__restrict__ X, int64_t ldx, int64_t units,
-                        NdhwcHostGeom g, int relu) {
-    host_reader_body<NS>(fmap, randx, randy, X, ldx, units, g, relu);
+                        HostGeom g, int relu) {
+    host_reader_body<NS, true>(fmap, randx, randy, X, ldx, units, g, relu);
 }
 
 }  // namespace
 
-// Channel chunk and stage sizes of the reader for a window of k2 taps and NS stages (G: NhwcHostGeom or
-// NdhwcHostGeom).  Returns false when one copy per tap does not fit a stage (never for the kh*kw <= 81 that
-// cp_patch_gather_conv, or the kt*kh*kw <= 343 that cp_patch_gather_conv3d, lets through).
-template <typename G>
-static bool host_chunks(G &g, const void *fmap, int esize, int c, int k2, int ns) {
+// Geometry, channel chunk and stage sizes of the reader for NS = ns stages.  Returns false when one copy per tap does
+// not fit a stage (never for the kh*kw <= 81 that cp_patch_gather_conv, or the kt*kh*kw <= 343 that
+// cp_patch_gather_conv3d, lets through).
+static bool host_geom(HostGeom &g, const void *fmap, int esize, int B, int P, int c, int D, int H, int W,
+                      const int32_t *randt, const cp_window &w, int ns) {
+    g.randt = randt, g.B = B, g.P = P, g.c = c, g.D = D, g.H = H, g.W = W, g.w = w;
+    const int k = w.kt * w.kh * w.kw;
     g.vec = (c * esize) % 16 == 0 && ((uintptr_t)fmap & 15) == 0;
     const int ve = g.vec ? 16 / esize : 1;
-    int ctmax = (NHWC_HOST_SMEM / ns / k2 - NHWC_HOST_PAD) / esize;
+    int ctmax = (NHWC_HOST_SMEM / ns / k - NHWC_HOST_PAD) / esize;
     ctmax -= ctmax % ve;
     if (ctmax < ve) return false;
     g.nchunk = cp_cdiv(c, ctmax);
     g.ct = cp_cdiv(cp_cdiv(c, g.nchunk), ve) * ve;  // balanced chunks, whole 16-byte copies
     g.nchunk = cp_cdiv(c, g.ct);
     g.tap = g.ct * esize + NHWC_HOST_PAD;
-    g.stage = k2 * g.tap;
+    g.stage = k * g.tap;
     return true;
 }
 
-static bool nhwc_host_geom(NhwcHostGeom &g, const void *fmap, int esize, int B, int P, int c, int H, int W,
-                           const cp_window &w, int ns) {
-    g.B = B, g.P = P, g.c = c, g.H = H, g.W = W, g.w = w;
-    return host_chunks(g, fmap, esize, c, w.kh * w.kw, ns);
-}
-
 template <int NS, typename T>
-static void launch_nhwc_host(const T *fmap, const NhwcHostGeom &g, int64_t rows, const int32_t *randx,
-                             const int32_t *randy, int relu, float *X_out, int64_t ldx, int ncta, cudaStream_t stream) {
+static void launch_host(const T *fmap, const HostGeom &g, int64_t rows, const int32_t *randx, const int32_t *randy,
+                        int relu, float *X_out, int64_t ldx, int ncta, cudaStream_t stream) {
     const int64_t units = rows * g.nchunk;
     const unsigned grid = (unsigned)(units < ncta ? units : ncta);
-    patch_gather_nhwc_host<NS, T><<<grid, 256, (size_t)NS * g.stage, stream>>>(fmap, randx, randy, X_out, ldx, units,
-                                                                                g, relu);
+    auto kern = g.randt ? patch_gather_ndhwc_host<NS, T> : patch_gather_nhwc_host<NS, T>;
+    kern<<<grid, 256, (size_t)NS * g.stage, stream>>>(fmap, randx, randy, X_out, ldx, units, g, relu);
 }
 
 // Grid and pipeline depth of the reader (profiles/host_nhwc_ctas.cu; H100 80GB HBM3 SXM, 700 W; DESIGN.md section 3).
@@ -255,45 +178,16 @@ static void launch_nhwc_host(const T *fmap, const NhwcHostGeom &g, int64_t rows,
 constexpr int CP_HOST_NHWC_GATHER_CTAS = 32;
 constexpr int CP_HOST_NHWC_STAGES = 2;
 
-int cp_patch_gather_nhwc_host(const void *fmap, int fmap_dtype, int nbatch, int B, int c, int H, int W,
-                              const int32_t *randx, const int32_t *randy, int P, const cp_window &w, int relu,
-                              float *X_out, int64_t ldx, cudaStream_t stream) {
-    NhwcHostGeom g;
-    CP_REQUIRE(nhwc_host_geom(g, fmap, cp_fmap_esize(fmap_dtype), B, P, c, H, W, w, CP_HOST_NHWC_STAGES),
-               "cp_patch_gather: kernel_size %dx%d too large for the NHWC host reader", w.kh, w.kw);
-    const int64_t rows = (int64_t)nbatch * P * B;
-    if (fmap_dtype == CP_F32)
-        launch_nhwc_host<CP_HOST_NHWC_STAGES>((const float *)fmap, g, rows, randx, randy, relu, X_out, ldx,
-                                              CP_HOST_NHWC_GATHER_CTAS, stream);
-    else if (fmap_dtype == CP_BF16)
-        launch_nhwc_host<CP_HOST_NHWC_STAGES>((const __nv_bfloat16 *)fmap, g, rows, randx, randy, relu, X_out, ldx,
-                                              CP_HOST_NHWC_GATHER_CTAS, stream);
-    else
-        launch_nhwc_host<CP_HOST_NHWC_STAGES>((const __half *)fmap, g, rows, randx, randy, relu, X_out, ldx,
-                                              CP_HOST_NHWC_GATHER_CTAS, stream);
-    CP_CHECK_LAUNCH();
-    return CP_OK;
-}
-
-int cp_patch_gather_ndhwc_host(const void *fmap, int fmap_dtype, int nbatch, int B, int c, int D, int H, int W,
-                               const int32_t *randt, const int32_t *randx, const int32_t *randy, int P,
-                               const cp_window3 &w, int relu, float *X_out, int64_t ldx, cudaStream_t stream) {
-    NdhwcHostGeom g;
-    g.randt = randt, g.B = B, g.P = P, g.c = c, g.D = D, g.H = H, g.W = W, g.w = w;
-    CP_REQUIRE(host_chunks(g, fmap, cp_fmap_esize(fmap_dtype), c, w.kt * w.kh * w.kw, CP_HOST_NHWC_STAGES),
-               "cp_patch_gather_conv3d: kernel_size %dx%dx%d too large for the NDHWC host reader", w.kt, w.kh, w.kw);
-    const int64_t units = (int64_t)nbatch * P * B * g.nchunk;
-    const unsigned grid = (unsigned)(units < CP_HOST_NHWC_GATHER_CTAS ? units : CP_HOST_NHWC_GATHER_CTAS);
-    const size_t smem = (size_t)CP_HOST_NHWC_STAGES * g.stage;
-    if (fmap_dtype == CP_F32)
-        patch_gather_ndhwc_host<CP_HOST_NHWC_STAGES><<<grid, 256, smem, stream>>>((const float *)fmap, randx, randy,
-                                                                                   X_out, ldx, units, g, relu);
-    else if (fmap_dtype == CP_BF16)
-        patch_gather_ndhwc_host<CP_HOST_NHWC_STAGES><<<grid, 256, smem, stream>>>(
-            (const __nv_bfloat16 *)fmap, randx, randy, X_out, ldx, units, g, relu);
-    else
-        patch_gather_ndhwc_host<CP_HOST_NHWC_STAGES><<<grid, 256, smem, stream>>>((const __half *)fmap, randx, randy,
-                                                                                   X_out, ldx, units, g, relu);
+int cp_patch_gather_host(const cp_patch_args &a) {
+    HostGeom g;
+    CP_REQUIRE(host_geom(g, a.fmap, cp_fmap_esize(a.dtype), a.B, a.P, a.c, a.D, a.H, a.W, a.randt, a.g,
+                         CP_HOST_NHWC_STAGES),
+               "%s: kernel_size %dx%dx%d too large for the channels-last host reader", a.name, a.g.kt, a.g.kh, a.g.kw);
+    cp_with_fmap_type(a.dtype, [&](auto z) {
+        using T = decltype(z);
+        launch_host<CP_HOST_NHWC_STAGES>((const T *)a.fmap, g, a.rows(), a.randx, a.randy, a.relu, a.X, a.ldx,
+                                         CP_HOST_NHWC_GATHER_CTAS, a.stream);
+    });
     CP_CHECK_LAUNCH();
     return CP_OK;
 }

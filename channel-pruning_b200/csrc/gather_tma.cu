@@ -1,4 +1,5 @@
-// Sparse-point im2col on NHWC feature maps, TMA in / TMA out -- the HBM-roofline path of cp_patch_gather
+// Sparse-point im2col on channels-last (NHWC / NDHWC) feature maps, TMA in / TMA out -- the HBM-roofline path of the
+// patch gathers
 // (replaces Net.extract_XY, reference lib/net.py:534-684, + the relu of lib/net.py:1720).
 //
 // One sampled output point needs a kh x kw x c window of the bottom blob (cp_window).  In NHWC that window is kh runs
@@ -19,8 +20,8 @@
 // bf16 / fp16 maps (template parameter T): the tensor map has the 16-bit data type, the window stage holds 16-bit
 // elements (half the bytes), and the consumers widen exactly while transposing; the row stays fp32.  6 N K bytes.
 // The 16-byte rules of TMA (global strides, box rows) then need c % 8 == 0.
-// NDHWC maps (Conv3d windows, cp_patch_gather_conv3d) take the same kernel body over a 5-D tensor map (c, W, H, D,
-// image): box (c_box, (kw-1)*dil_w+1, (kh-1)*dil_h+1, (kt-1)*dil_t+1, 1), traversal strides (1, dil_w, dil_h, dil_t, 1),
+// NDHWC maps (Conv3d windows) take the same kernel body (ND = 5) over a 5-D tensor map (c, W, H, D, image): box
+// (c_box, (kw-1)*dil_w+1, (kh-1)*dil_h+1, (kt-1)*dil_t+1, 1), traversal strides (1, dil_w, dil_h, dil_t, 1),
 // one cp.async.bulk.tensor.5d request per box delivering kt x kh x kw taps per channel.  A 3 x 3 x 3 window is three
 // times a 3 x 3 one, so there a work unit is one channel box of a row rather than the whole row: the stage and the
 // output segment (c_box kt kh kw contiguous floats of X) keep the size of the 2-D conv4_x rows.
@@ -212,13 +213,14 @@ __device__ __forceinline__ void gt_body(const CUtensorMap &map, const GtParams &
     if (tid == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // shared memory must outlive the reads
 }
 
-template <typename T, int K2>  // map element type; kh*kw known at compile time (1, 9, 25) or 0
+// The kernel by name, one per rank of the tensor map (profiles and tests tell the paths apart by it); T: map element
+// type; K2: taps known at compile time (gt_launch) or 0
+template <typename T, int K2>
 __global__ void __launch_bounds__(GT_THREADS)
 patch_gather_nhwc_tma(const __grid_constant__ CUtensorMap map, const GtParams P) {
     gt_body<T, K2, 4>(map, P);
 }
-
-template <typename T, int K2>  // map element type; kt*kh*kw known at compile time (1, 9, 27) or 0
+template <typename T, int K2>
 __global__ void __launch_bounds__(GT_THREADS)
 patch_gather_ndhwc_tma(const __grid_constant__ CUtensorMap map, const GtParams P) {
     gt_body<T, K2, 5>(map, P);
@@ -242,6 +244,14 @@ typedef CUresult (*encode_fn_t)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, 
 
 typedef void (*gt_kernel_t)(const CUtensorMap, const GtParams);
 
+template <int ND, typename T, int K2>
+static gt_kernel_t gt_kernel() {
+    if constexpr (ND == 4)
+        return patch_gather_nhwc_tma<T, K2>;
+    else
+        return patch_gather_ndhwc_tma<T, K2>;
+}
+
 static int gt_run(cp_handle_t h, gt_kernel_t kern, cp_per_device_flag &configured, const CUtensorMap &map,
                   const GtParams &Pm, size_t smem, int per_sm, cudaStream_t stream) {
     if (bool *done = configured.slot(); !*done) {
@@ -255,27 +265,17 @@ static int gt_run(cp_handle_t h, gt_kernel_t kern, cp_per_device_flag &configure
     return CP_OK;
 }
 
-template <typename T>
+// One instantiation per (rank, element type, taps): 1 x 1 and 3 x 3 windows of either rank, 5 x 5 of 2-D maps and
+// 3 x 3 x 3 of 3-D maps at compile time (a dilated window takes the instantiation of its tap count), the rest K2 = 0
+template <int ND, typename T>
 static int gt_launch(cp_handle_t h, const CUtensorMap &map, const GtParams &Pm, size_t smem, int per_sm,
                      cudaStream_t stream) {
-    // the consumers only see the number of taps: a dilated 3 x 3 window takes the 3 x 3 instantiation
+    constexpr int KBIG = ND == 4 ? 25 : 27;
     const int k2 = Pm.k2;
-    auto kern = k2 == 9 ? patch_gather_nhwc_tma<T, 9> : k2 == 1 ? patch_gather_nhwc_tma<T, 1>
-              : k2 == 25 ? patch_gather_nhwc_tma<T, 25> : patch_gather_nhwc_tma<T, 0>;
-    static cp_per_device_flag configured[4];  // one set per element type (one per instantiation of gt_launch)
-    const int which = k2 == 9 ? 0 : k2 == 1 ? 1 : k2 == 25 ? 2 : 3;
-    return gt_run(h, kern, configured[which], map, Pm, smem, per_sm, stream);
-}
-
-template <typename T>
-static int gt_launch3d(cp_handle_t h, const CUtensorMap &map, const GtParams &Pm, size_t smem, int per_sm,
-                       cudaStream_t stream) {
-    // 3 x 3 x 3, 1 x 3 x 3 (the spatial half of R(2+1)D) and 1 x 1 x 1 at compile time
-    const int k2 = Pm.k2;
-    auto kern = k2 == 27 ? patch_gather_ndhwc_tma<T, 27> : k2 == 9 ? patch_gather_ndhwc_tma<T, 9>
-              : k2 == 1 ? patch_gather_ndhwc_tma<T, 1> : patch_gather_ndhwc_tma<T, 0>;
-    static cp_per_device_flag configured[4];
-    const int which = k2 == 27 ? 0 : k2 == 9 ? 1 : k2 == 1 ? 2 : 3;
+    auto kern = k2 == 9 ? gt_kernel<ND, T, 9>() : k2 == 1 ? gt_kernel<ND, T, 1>()
+              : k2 == KBIG ? gt_kernel<ND, T, KBIG>() : gt_kernel<ND, T, 0>();
+    static cp_per_device_flag configured[4];  // one set per (rank, element type): one per instantiation of gt_launch
+    const int which = k2 == 9 ? 0 : k2 == 1 ? 1 : k2 == KBIG ? 2 : 3;
     return gt_run(h, kern, configured[which], map, Pm, smem, per_sm, stream);
 }
 
@@ -308,155 +308,115 @@ static CUtensorMapDataType gt_dtype(int fmap_dtype) {
                                   : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
 }
 
-// Channels per TMA box: the largest divisor of c in [16, 256] whose box row is a multiple of 16 bytes (TMA), 0 if none
-static int gt_cbox(int c, int esize) {
-    for (int d = 256; d >= 16; d -= 16 / esize)
-        if (c % d == 0) return d;
-    return 0;
-}
-
-// Traversal strides of a tensor map are at most 8 and box extents at most 256 (cuTensorMapEncodeTiled)
-constexpr int GT_MAX_DIL = 8, GT_MAX_SPAN = 256;
-
-// true when the TMA path applies (device memory, 16-byte rules, dilation <= 8, window spans <= 256, extents <= 16);
-// the caller falls back to the SIMT kernel otherwise
-bool cp_gather_tma_eligible(const void *fmap, int esize, int c, const cp_window &g, float *X_out, int64_t ldx) {
-    if (c % (16 / esize) || c < 16 || g.kh > 16 || g.kw > 16) return false;
-    if (g.dil_h > GT_MAX_DIL || g.dil_w > GT_MAX_DIL) return false;
-    if ((g.kh - 1) * g.dil_h + 1 > GT_MAX_SPAN || (g.kw - 1) * g.dil_w + 1 > GT_MAX_SPAN) return false;
-    const int k2 = g.kh * g.kw;
-    if (((uintptr_t)fmap & 15) || ((uintptr_t)X_out & 15) || (ldx % 4)) return false;
-    cudaPointerAttributes pa;
-    if (cudaPointerGetAttributes(&pa, fmap) != cudaSuccess || pa.type != cudaMemoryTypeDevice) {
-        (void)cudaGetLastError();
-        return false;
-    }
-    const int cbox = gt_cbox(c, esize);
-    if (!cbox) return false;
-    // a window stage and an output row; for fp32 the stage is never smaller than the row
-    const size_t row = gt_round128((size_t)cbox * k2 * esize) * (c / cbox);
-    const size_t out_b = gt_round128((size_t)c * k2 * 4);
-    return 2 * row + GT_OUT * (row > out_b ? row : out_b) + 1024 <= 200 * 1024;  // at least two input stages in one CTA
-}
-
-int cp_patch_gather_tma(cp_handle_t h, const void *fmap, int fmap_dtype, int nbatch, int B, int c, int H, int W,
-                        const int32_t *randx, const int32_t *randy, int P, const cp_window &g, int relu,
-                        float *X_out, int64_t ldx, cudaStream_t stream) {
-    if (int rc = gt_encode_fn(h)) return rc;
-    const int esize = cp_fmap_esize(fmap_dtype);
-    const int cbox = gt_cbox(c, esize);
-    const int64_t nimg = (int64_t)nbatch * B;
-    CUtensorMap map;
-    const cuuint64_t dims[4] = {(cuuint64_t)c, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)nimg};
-    const cuuint64_t strides[3] = {(cuuint64_t)c * esize, (cuuint64_t)W * c * esize, (cuuint64_t)H * W * c * esize};
-    // the box spans the dilated window; the traversal strides pick its kw x kh taps, which land densely
-    const cuuint32_t box[4] = {(cuuint32_t)cbox, (cuuint32_t)((g.kw - 1) * g.dil_w + 1),
-                               (cuuint32_t)((g.kh - 1) * g.dil_h + 1), 1};
-    const cuuint32_t estr[4] = {1, (cuuint32_t)g.dil_w, (cuuint32_t)g.dil_h, 1};
-    CUresult cr = ((encode_fn_t)h->tmap_encode)(&map, gt_dtype(fmap_dtype), 4, (void *)fmap, dims, strides, box, estr,
-                                                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-                                                CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) CP_FAIL(CP_ERR_CUDA, "cuTensorMapEncodeTiled (4-D feature map) failed (%d)", (int)cr);
-    GtParams Pm{};
-    Pm.randx = randx; Pm.randy = randy; Pm.X = X_out; Pm.ldx = ldx;
-    Pm.rows = (int64_t)nbatch * P * B;
-    const int k2 = g.kh * g.kw;
-    Pm.B = B; Pm.P = P; Pm.c = c; Pm.k2 = k2; Pm.relu = relu;
-    Pm.pad_h = g.pad_h; Pm.pad_w = g.pad_w; Pm.stride_h = g.stride_h; Pm.stride_w = g.stride_w;
-    Pm.cbox = cbox; Pm.nbox = c / cbox;
-    // Bytes the copy engine delivers per box, hence what expect_tx must announce (the kernel arms c * k2 * esize per
-    // window): ceil(box[i] / estr[i]) elements per dimension, i.e. cbox x kw x kh x 1 (gt_box_elems).
-    const size_t box_b = gt_round128(gt_box_elems(box, estr, 4) * esize), row = box_b * Pm.nbox;
-    if (gt_box_elems(box, estr, 4) != (size_t)cbox * k2)
-        CP_FAIL(CP_ERR_CUDA, "cp_patch_gather: TMA box delivers %zu elements, the window has %zu",
-                gt_box_elems(box, estr, 4), (size_t)cbox * k2);
-    const size_t out_b = gt_round128((size_t)c * k2 * 4);
-    int per_sm, nstage;
-    gt_ring(row, out_b, per_sm, nstage);
-    Pm.nstage = nstage;
-    Pm.box_f = (int)(box_b / esize); Pm.stage_f = (int)(row / esize); Pm.out_f = (int)(out_b / 4);
-    const size_t smem = (size_t)nstage * row + GT_OUT * out_b + 2 * nstage * 8 + 256;
-    if (fmap_dtype == CP_BF16) return gt_launch<__nv_bfloat16>(h, map, Pm, smem, per_sm, stream);
-    if (fmap_dtype == CP_F16) return gt_launch<__half>(h, map, Pm, smem, per_sm, stream);
-    return gt_launch<float>(h, map, Pm, smem, per_sm, stream);
-}
-
-// ---------------------------------------------------------------------------------------------------- 5-D (NDHWC)
-
 // Bytes of one work unit's output segment the 3-D path aims at: the fp32 row of the 2-D path at conv4_x (c = 512,
 // 3 x 3), which that path moves at its best rate.  A 3 x 3 x 3 window at c >= 128 is split into 128-channel units.
 constexpr size_t GT3_UNIT_BYTES = 18 * 1024;
 
-// Channels per box (= per work unit) of the 3-D path: the largest divisor of c in [16, 256] with whole 16-byte box rows
-// whose fp32 output segment is at most GT3_UNIT_BYTES; the smallest such divisor when none is; 0 when c has none
-static int gt_cbox3d(int c, int esize, int k3) {
+// Channels per TMA box: the largest divisor d of c in [16, 256] with whole 16-byte box rows (TMA) whose fp32 output
+// segment d * taps * 4 is at most seg_max bytes; the smallest such divisor when none is; 0 when c has none
+static int gt_cbox(int c, int esize, int taps, size_t seg_max) {
     int last = 0;
     for (int d = 256; d >= 16; d -= 16 / esize) {
         if (c % d) continue;
-        if ((size_t)d * k3 * 4 <= GT3_UNIT_BYTES) return d;
+        if ((size_t)d * taps * 4 <= seg_max) return d;
         last = d;
     }
     return last;
 }
 
-bool cp_gather_tma3d_eligible(const void *fmap, int esize, int c, const cp_window3 &g, float *X_out, int64_t ldx) {
+// Traversal strides of a tensor map are at most 8 and box extents at most 256 (cuTensorMapEncodeTiled)
+constexpr int GT_MAX_DIL = 8, GT_MAX_SPAN = 256;
+
+// How a channels-last map goes through the kernel.  2-D maps: a rank-4 tensor map, a work unit is a whole row of X
+// (nbox = c / cbox boxes, gt_cbox's largest box).  3-D maps: a rank-5 tensor map, a work unit is one box of a row
+// (ngrp = c / cbox units per row), the box sized by GT3_UNIT_BYTES.
+struct GtPlan {
+    int rank, taps, cbox, uc, nbox, ngrp;  // uc: channels per unit
+    size_t box_b, row, out_b;             // bytes of a box and of a unit's window stage (type T) and output (fp32)
+    int per_sm, nstage;
+    size_t smem;
+};
+
+// false when the TMA path does not take the window: the 16-byte rules, an extent over 16, a dilation over 8, a span
+// over 256, no channel box, or no room for two input stages in one CTA
+static bool gt_plan(GtPlan &pl, int esize, int c, const cp_window &g, bool depth) {
     if (c % (16 / esize) || c < 16 || g.kt > 16 || g.kh > 16 || g.kw > 16) return false;
     if (g.dil_t > GT_MAX_DIL || g.dil_h > GT_MAX_DIL || g.dil_w > GT_MAX_DIL) return false;
     if ((g.kt - 1) * g.dil_t + 1 > GT_MAX_SPAN || (g.kh - 1) * g.dil_h + 1 > GT_MAX_SPAN ||
         (g.kw - 1) * g.dil_w + 1 > GT_MAX_SPAN)
         return false;
-    if (((uintptr_t)fmap & 15) || ((uintptr_t)X_out & 15) || (ldx % 4)) return false;
-    cudaPointerAttributes pa;
-    if (cudaPointerGetAttributes(&pa, fmap) != cudaSuccess || pa.type != cudaMemoryTypeDevice) {
-        (void)cudaGetLastError();
-        return false;
-    }
-    const int k3 = g.kt * g.kh * g.kw;
-    const int cbox = gt_cbox3d(c, esize, k3);
-    if (!cbox) return false;
-    const size_t row = gt_round128((size_t)cbox * k3 * esize), out_b = gt_round128((size_t)cbox * k3 * 4);
-    return 2 * row + GT_OUT * (row > out_b ? row : out_b) + 1024 <= 200 * 1024;
+    pl.rank = depth ? 5 : 4;
+    pl.taps = g.kt * g.kh * g.kw;
+    pl.cbox = gt_cbox(c, esize, pl.taps, depth ? GT3_UNIT_BYTES : SIZE_MAX);
+    if (!pl.cbox) return false;
+    pl.uc = depth ? pl.cbox : c;
+    pl.nbox = pl.uc / pl.cbox;
+    pl.ngrp = c / pl.uc;
+    pl.box_b = gt_round128((size_t)pl.cbox * pl.taps * esize);
+    pl.row = pl.box_b * pl.nbox;
+    pl.out_b = gt_round128((size_t)pl.uc * pl.taps * 4);
+    // for fp32 the stage is never smaller than the output
+    if (2 * pl.row + GT_OUT * (pl.row > pl.out_b ? pl.row : pl.out_b) + 1024 > 200 * 1024) return false;
+    gt_ring(pl.row, pl.out_b, pl.per_sm, pl.nstage);
+    pl.smem = (size_t)pl.nstage * pl.row + GT_OUT * pl.out_b + 2 * pl.nstage * 8 + 256;
+    return true;
 }
 
-int cp_patch_gather_tma3d(cp_handle_t h, const void *fmap, int fmap_dtype, int nbatch, int B, int c, int D, int H,
-                          int W, const int32_t *randt, const int32_t *randx, const int32_t *randy, int P,
-                          const cp_window3 &g, int relu, float *X_out, int64_t ldx, cudaStream_t stream) {
-    if (int rc = gt_encode_fn(h)) return rc;
-    const int esize = cp_fmap_esize(fmap_dtype);
-    const int k3 = g.kt * g.kh * g.kw;
-    const int cbox = gt_cbox3d(c, esize, k3);
-    const int64_t nimg = (int64_t)nbatch * B;
-    CUtensorMap map;
-    const cuuint64_t dims[5] = {(cuuint64_t)c, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)D, (cuuint64_t)nimg};
-    const cuuint64_t pix = (cuuint64_t)c * esize;
-    const cuuint64_t strides[4] = {pix, W * pix, (cuuint64_t)H * W * pix, (cuuint64_t)D * H * W * pix};
-    // the box spans the dilated window; the traversal strides pick its kw x kh x kt taps, which land densely
-    const cuuint32_t box[5] = {(cuuint32_t)cbox, (cuuint32_t)((g.kw - 1) * g.dil_w + 1),
+// The tensor map over (c, W, H, image) or (c, W, H, D, image).  The box spans the dilated window,
+// (cbox, (kw-1)*dil_w+1, (kh-1)*dil_h+1[, (kt-1)*dil_t+1], 1); the traversal strides (1, dil_w, dil_h[, dil_t], 1)
+// pick its taps, which land densely.
+static int gt_encode(cp_handle_t h, CUtensorMap &map, const cp_patch_args &a, const GtPlan &pl) {
+    const cp_window &g = a.g;
+    const int esize = cp_fmap_esize(a.dtype), n = pl.rank;
+    cuuint64_t dims[5] = {(cuuint64_t)a.c, (cuuint64_t)a.W, (cuuint64_t)a.H, (cuuint64_t)a.D,
+                          (cuuint64_t)a.nbatch * a.B};
+    if (n == 4) dims[3] = dims[4];  // no depth axis
+    cuuint64_t strides[4] = {(cuuint64_t)a.c * esize};
+    for (int i = 1; i < n - 1; ++i) strides[i] = strides[i - 1] * dims[i];
+    const cuuint32_t box[5] = {(cuuint32_t)pl.cbox, (cuuint32_t)((g.kw - 1) * g.dil_w + 1),
                                (cuuint32_t)((g.kh - 1) * g.dil_h + 1), (cuuint32_t)((g.kt - 1) * g.dil_t + 1), 1};
     const cuuint32_t estr[5] = {1, (cuuint32_t)g.dil_w, (cuuint32_t)g.dil_h, (cuuint32_t)g.dil_t, 1};
-    CUresult cr = ((encode_fn_t)h->tmap_encode)(&map, gt_dtype(fmap_dtype), 5, (void *)fmap, dims, strides, box, estr,
+    CUresult cr = ((encode_fn_t)h->tmap_encode)(&map, gt_dtype(a.dtype), n, (void *)a.fmap, dims, strides, box, estr,
                                                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
                                                 CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) CP_FAIL(CP_ERR_CUDA, "cuTensorMapEncodeTiled (5-D feature map) failed (%d)", (int)cr);
-    // expect_tx announces cbox * kt * kh * kw elements per unit: what the copy engine delivers by the ceil rule
-    if (gt_box_elems(box, estr, 5) != (size_t)cbox * k3)
-        CP_FAIL(CP_ERR_CUDA, "cp_patch_gather_conv3d: TMA box delivers %zu elements, the window has %zu",
-                gt_box_elems(box, estr, 5), (size_t)cbox * k3);
+    if (cr != CUDA_SUCCESS) CP_FAIL(CP_ERR_CUDA, "cuTensorMapEncodeTiled (%d-D feature map) failed (%d)", n, (int)cr);
+    // Elements the copy engine delivers per box, hence what expect_tx must announce (the kernel arms cbox * taps per
+    // box): ceil(box[i] / estr[i]) per dimension (gt_box_elems)
+    if (gt_box_elems(box, estr, n) != (size_t)pl.cbox * pl.taps)
+        CP_FAIL(CP_ERR_CUDA, "%s: TMA box delivers %zu elements, the window has %zu", a.name, gt_box_elems(box, estr, n),
+                (size_t)pl.cbox * pl.taps);
+    return CP_OK;
+}
+
+// true when the TMA path takes a channels-last map that lies in device memory: 16-byte aligned fmap, X_out and ldx,
+// and a plan (gt_plan); the caller takes the SIMT kernel otherwise
+bool cp_gather_tma_applies(const cp_patch_args &a) {
+    if (((uintptr_t)a.fmap & 15) || ((uintptr_t)a.X & 15) || (a.ldx % 4)) return false;
+    GtPlan pl;
+    return gt_plan(pl, cp_fmap_esize(a.dtype), a.c, a.g, a.randt != nullptr);
+}
+
+int cp_patch_gather_tma(cp_handle_t h, const cp_patch_args &a) {
+    const int esize = cp_fmap_esize(a.dtype);
+    GtPlan pl;
+    if (!gt_plan(pl, esize, a.c, a.g, a.randt != nullptr))
+        CP_FAIL(CP_ERR_INVALID, "%s: the window does not fit the TMA path", a.name);
+    if (int rc = gt_encode_fn(h)) return rc;
+    CUtensorMap map;
+    if (int rc = gt_encode(h, map, a, pl)) return rc;
+    const cp_window &g = a.g;
     GtParams Pm{};
-    Pm.randx = randx; Pm.randy = randy; Pm.randt = randt; Pm.X = X_out; Pm.ldx = ldx;
-    Pm.ngrp = c / cbox;
-    Pm.rows = (int64_t)nbatch * P * B * Pm.ngrp;  // work units
-    Pm.B = B; Pm.P = P; Pm.c = cbox; Pm.k2 = k3; Pm.relu = relu;
+    Pm.randx = a.randx; Pm.randy = a.randy; Pm.randt = a.randt; Pm.X = a.X; Pm.ldx = a.ldx;
+    Pm.ngrp = pl.ngrp;
+    Pm.rows = a.rows() * pl.ngrp;  // work units
+    Pm.B = a.B; Pm.P = a.P; Pm.c = pl.uc; Pm.k2 = pl.taps; Pm.relu = a.relu;
     Pm.pad_t = g.pad_t; Pm.pad_h = g.pad_h; Pm.pad_w = g.pad_w;
     Pm.stride_t = g.stride_t; Pm.stride_h = g.stride_h; Pm.stride_w = g.stride_w;
-    Pm.cbox = cbox; Pm.nbox = 1;
-    const size_t row = gt_round128((size_t)cbox * k3 * esize), out_b = gt_round128((size_t)cbox * k3 * 4);
-    int per_sm, nstage;
-    gt_ring(row, out_b, per_sm, nstage);
-    Pm.nstage = nstage;
-    Pm.box_f = (int)(row / esize); Pm.stage_f = Pm.box_f; Pm.out_f = (int)(out_b / 4);
-    const size_t smem = (size_t)nstage * row + GT_OUT * out_b + 2 * nstage * 8 + 256;
-    if (fmap_dtype == CP_BF16) return gt_launch3d<__nv_bfloat16>(h, map, Pm, smem, per_sm, stream);
-    if (fmap_dtype == CP_F16) return gt_launch3d<__half>(h, map, Pm, smem, per_sm, stream);
-    return gt_launch3d<float>(h, map, Pm, smem, per_sm, stream);
+    Pm.cbox = pl.cbox; Pm.nbox = pl.nbox; Pm.nstage = pl.nstage;
+    Pm.box_f = (int)(pl.box_b / esize); Pm.stage_f = (int)(pl.row / esize); Pm.out_f = (int)(pl.out_b / 4);
+    return cp_with_fmap_type(a.dtype, [&](auto z) {
+        using T = decltype(z);
+        return pl.rank == 5 ? gt_launch<5, T>(h, map, Pm, pl.smem, pl.per_sm, a.stream)
+                            : gt_launch<4, T>(h, map, Pm, pl.smem, pl.per_sm, a.stream);
+    });
 }

@@ -60,6 +60,17 @@ def fmap_dtype_code(dtype):
     return code
 
 
+def _gather_map(fmap, B, layout, d3):
+    """(dtype code, layout code, nbatch, dims) of a gather's map (nbatch*B images): dims is (c, H, W) of a 2-D map and
+    (c, D, H, W) of a 3-D one (d3), c the channels whichever the layout.  TypeError for a dtype the gathers do not read,
+    before anything else."""
+    dt = fmap_dtype_code(fmap.dtype)
+    assert fmap.is_contiguous() and fmap.dim() == (5 if d3 else 4)
+    lay = (_LAYOUTS3D if d3 else _LAYOUTS)[layout]
+    s = tuple(fmap.shape[1:])
+    return dt, lay, fmap.shape[0] // B, s if lay == 0 else s[-1:] + s[:-1]
+
+
 class LassoResult:
     """Device-resident outputs of one channel selection (cp_lasso_select)."""
 
@@ -254,49 +265,18 @@ class Engine:
         k, pad, stride, dilation: an int or an (h, w) pair, with the meaning of torch.nn.Conv2d's arguments (pad: the
         top / left padding; the sampled points already respect the output size).  Columns are in F.unfold's order.
         All ints with dilation 1 is the reference's window, which must be odd (an even square kernel is (k, k))."""
-        dt = fmap_dtype_code(fmap.dtype)
-        assert fmap.is_contiguous()
-        nimg = fmap.shape[0]
-        assert nimg % B == 0
-        nbatch = nimg // B
-        if layout == "nchw":
-            c, H, W = fmap.shape[1], fmap.shape[2], fmap.shape[3]
-        else:
-            H, W, c = fmap.shape[1], fmap.shape[2], fmap.shape[3]
-        assert randx.dtype == torch.int32 and randx.numel() == nbatch * P and randx.is_contiguous()
-        assert randy.dtype == torch.int32 and randy.numel() == nbatch * P and randy.is_contiguous()
+        geo = _gather_map(fmap, B, layout, False)
         (kh, kw), (ph, pw), (sh, sw), (dh, dw) = (conv_pair(v) for v in (k, pad, stride, dilation))
-        rows, K = nbatch * P * B, c * kh * kw
-        if out is None:
-            out = self.empty(rows, K, dtype=torch.float32)
-        assert out.shape == (rows, K) and out.dtype == torch.float32 and out.stride(1) == 1
-        args = (self.h, self._p(fmap, "const void*"), dt, nbatch, B, c, H, W, _LAYOUTS[layout],
-                self._p(randx, "const int32_t*"), self._p(randy, "const int32_t*"), P)
-        tail = (int(bool(relu)), self._p(out, "float*"), out.stride(0), self._s())
         if all(isinstance(v, (int, np.integer)) for v in (k, pad, stride, dilation)) and dilation == 1:
-            self._call(self.lib.cp_patch_gather_typed(*args, kh, ph, sh, *tail))
+            fn, window = self.lib.cp_patch_gather_typed, (kh, ph, sh)
         else:
-            self._call(self.lib.cp_patch_gather_conv(*args, kh, kw, ph, pw, sh, sw, dh, dw, *tail))
-        return out
+            fn, window = self.lib.cp_patch_gather_conv, (kh, kw, ph, pw, sh, sw, dh, dw)
+        return self._patch_gather(fn, geo, fmap, (randx, randy), B, P, kh * kw, window, relu, out)
 
     def point_gather(self, fmap, randx, randy, B, P, layout="nchw", out=None):
         """Y (nbatch*P*B, n) fp32 at the sampled points of fmap (float32 / bfloat16 / float16, widened exactly)."""
-        dt = fmap_dtype_code(fmap.dtype)
-        assert fmap.is_contiguous()
-        nimg = fmap.shape[0]
-        nbatch = nimg // B
-        if layout == "nchw":
-            n, H, W = fmap.shape[1], fmap.shape[2], fmap.shape[3]
-        else:
-            H, W, n = fmap.shape[1], fmap.shape[2], fmap.shape[3]
-        rows = nbatch * P * B
-        if out is None:
-            out = self.empty(rows, n, dtype=torch.float32)
-        self._call(self.lib.cp_point_gather_typed(self.h, self._p(fmap, "const void*"), dt, nbatch, B, n, H, W,
-                                                  _LAYOUTS[layout], self._p(randx, "const int32_t*"),
-                                                  self._p(randy, "const int32_t*"), P, self._p(out, "float*"),
-                                                  out.stride(0), self._s()))
-        return out
+        geo = _gather_map(fmap, B, layout, False)
+        return self._point_gather(self.lib.cp_point_gather_typed, geo, fmap, (randx, randy), B, P, out)
 
     def patch_gather3d(self, fmap, randt, randx, randy, B, P, k, pad, stride, relu=True, layout="ncdhw", out=None,
                        dilation=1):
@@ -305,47 +285,43 @@ class Engine:
         device, the sampled output points (t, x, y).  Returns X (nbatch*P*B, c*kt*kh*kw) fp32, 16-bit maps widened
         exactly.  k, pad, stride, dilation: an int or a (t, h, w) triple, with the meaning of torch.nn.Conv3d's
         arguments (pad: the front / top / left padding).  Columns are in Conv3d.weight.reshape(n, -1)'s order."""
-        dt = fmap_dtype_code(fmap.dtype)
-        assert fmap.is_contiguous() and fmap.dim() == 5
-        nimg = fmap.shape[0]
-        assert nimg % B == 0
-        nbatch = nimg // B
-        if layout == "ncdhw":
-            c, D, H, W = fmap.shape[1:]
-        else:
-            D, H, W, c = fmap.shape[1:]
-        for r in (randt, randx, randy):
-            assert r.dtype == torch.int32 and r.numel() == nbatch * P and r.is_contiguous()
-        (kt, kh, kw), (pt, ph, pw), (st, sh, sw), (dt_, dh, dw) = (conv_triple(v) for v in (k, pad, stride, dilation))
-        rows, K = nbatch * P * B, c * kt * kh * kw
-        if out is None:
-            out = self.empty(rows, K, dtype=torch.float32)
-        assert out.shape == (rows, K) and out.dtype == torch.float32 and out.stride(1) == 1
-        self._call(self.lib.cp_patch_gather_conv3d(
-            self.h, self._p(fmap, "const void*"), dt, nbatch, B, c, D, H, W, _LAYOUTS3D[layout],
-            self._p(randt, "const int32_t*"), self._p(randx, "const int32_t*"), self._p(randy, "const int32_t*"), P,
-            kt, kh, kw, pt, ph, pw, st, sh, sw, dt_, dh, dw, int(bool(relu)), self._p(out, "float*"), out.stride(0),
-            self._s()))
-        return out
+        geo = _gather_map(fmap, B, layout, True)
+        (kt, kh, kw), (pt, ph, pw), (st, sh, sw), (dt, dh, dw) = (conv_triple(v) for v in (k, pad, stride, dilation))
+        return self._patch_gather(self.lib.cp_patch_gather_conv3d, geo, fmap, (randt, randx, randy), B, P,
+                                  kt * kh * kw, (kt, kh, kw, pt, ph, pw, st, sh, sw, dt, dh, dw), relu, out)
 
     def point_gather3d(self, fmap, randt, randx, randy, B, P, layout="ncdhw", out=None):
         """Y (nbatch*P*B, n) fp32 at the sampled points (t, x, y) of a Conv3d output map (nbatch*B, n, To, Ho, Wo)
         [ncdhw] or (nbatch*B, To, Ho, Wo, n) [ndhwc], float32 / bfloat16 / float16 widened exactly."""
-        dt = fmap_dtype_code(fmap.dtype)
-        assert fmap.is_contiguous() and fmap.dim() == 5
-        nbatch = fmap.shape[0] // B
-        if layout == "ncdhw":
-            n, D, H, W = fmap.shape[1:]
-        else:
-            D, H, W, n = fmap.shape[1:]
-        rows = nbatch * P * B
+        geo = _gather_map(fmap, B, layout, True)
+        return self._point_gather(self.lib.cp_point_gather3d, geo, fmap, (randt, randx, randy), B, P, out)
+
+    def _patch_gather(self, fn, geo, fmap, points, B, P, taps, window, relu, out):
+        """patch_gather and patch_gather3d from here on: fn is the C entry, geo what _gather_map found, points the
+        (randx, randy) or (randt, randx, randy) tensors, window the entry's geometry arguments."""
+        dt, lay, nbatch, dims = geo
+        assert fmap.shape[0] % B == 0
+        for r in points:
+            assert r.dtype == torch.int32 and r.numel() == nbatch * P and r.is_contiguous()
+        rows, K = nbatch * P * B, dims[0] * taps
+        if out is None:
+            out = self.empty(rows, K, dtype=torch.float32)
+        assert out.shape == (rows, K) and out.dtype == torch.float32 and out.stride(1) == 1
+        self._call(fn(self.h, self._p(fmap, "const void*"), dt, nbatch, B, *dims, lay,
+                      *[self._p(r, "const int32_t*") for r in points], P, *window, int(bool(relu)),
+                      self._p(out, "float*"), out.stride(0), self._s()))
+        return out
+
+    def _point_gather(self, fn, geo, fmap, points, B, P, out):
+        """point_gather and point_gather3d from here on (arguments as for _patch_gather)."""
+        dt, lay, nbatch, dims = geo
+        rows, n = nbatch * P * B, dims[0]
         if out is None:
             out = self.empty(rows, n, dtype=torch.float32)
         assert out.shape == (rows, n) and out.dtype == torch.float32 and out.stride(1) == 1
-        self._call(self.lib.cp_point_gather3d(
-            self.h, self._p(fmap, "const void*"), dt, nbatch, B, n, D, H, W, _LAYOUTS3D[layout],
-            self._p(randt, "const int32_t*"), self._p(randx, "const int32_t*"), self._p(randy, "const int32_t*"), P,
-            self._p(out, "float*"), out.stride(0), self._s()))
+        self._call(fn(self.h, self._p(fmap, "const void*"), dt, nbatch, B, *dims, lay,
+                      *[self._p(r, "const int32_t*") for r in points], P, self._p(out, "float*"), out.stride(0),
+                      self._s()))
         return out
 
     def gram(self, X, Y=None, y_bias=None, rows=None, want_G=True, want_B=True, want_sums=True, want_yy=False,

@@ -130,9 +130,11 @@ int cp_patch_gather_typed(cp_handle_t h, const void *fmap, int fmap_dtype, int n
  * CP_ERR_INVALID before any device work.
  * Paths, as for the square window: NHWC in device memory takes the TMA kernel when its 16-byte rules hold, both
  * dilations are <= 8, both window spans (k-1)*dil+1 are <= 256 and kh, kw <= 16; other NHWC device maps take the
- * SIMT kernel (kh*kw <= 95: its shared-memory tile); NHWC maps in pinned host memory take the in-place reader
- * (kh*kw <= 81); NCHW maps take the SIMT kernel with any window.  A window beyond a path's bound returns
- * CP_ERR_INVALID.  Square, odd, undilated windows give the bits of cp_patch_gather_typed.
+ * SIMT kernel (kh*kw <= 95); NHWC maps in pinned host memory take the in-place reader (kh*kw <= 81); NCHW maps take
+ * the SIMT kernel with any window.  A window beyond a path's bound returns CP_ERR_INVALID.  The two bounds are the
+ * contract of the 2-D entries (cp_patch_gather, _typed, _conv), kept from their square windows: the kernels are those
+ * of cp_patch_gather_conv3d, which takes larger windows.  Square, odd, undilated windows give the bits of
+ * cp_patch_gather_typed.
  */
 int cp_patch_gather_conv(cp_handle_t h, const void *fmap, int fmap_dtype, int nbatch, int B, int c, int H, int W,
                          int layout, const int32_t *randx, const int32_t *randy, int P, int kh, int kw, int pad_h,

@@ -26,15 +26,15 @@ struct Layer {
 };
 
 template <int NS, typename T>
-static float run(const T *map, const NhwcHostGeom &g0, int64_t rows, const int32_t *rx, const int32_t *ry, float *X,
+static float run(const T *map, const HostGeom &g0, int64_t rows, const int32_t *rx, const int32_t *ry, float *X,
                  int64_t ldx, int ncta, int launches) {
-    NhwcHostGeom g;
-    if (!nhwc_host_geom(g, map, (int)sizeof(T), g0.B, g0.P, g0.c, g0.H, g0.W, g0.k, g0.pad, g0.stride, NS)) exit(2);
+    HostGeom g;
+    if (!host_geom(g, map, (int)sizeof(T), g0.B, g0.P, g0.c, 1, g0.H, g0.W, nullptr, g0.w, NS)) exit(2);
     cudaEvent_t a, b;
     CK(cudaEventCreate(&a));
     CK(cudaEventCreate(&b));
     CK(cudaEventRecord(a));
-    for (int i = 0; i < launches; ++i) launch_nhwc_host<NS>(map, g, rows, rx, ry, 1, X, ldx, ncta, 0);
+    for (int i = 0; i < launches; ++i) launch_host<NS>(map, g, rows, rx, ry, 1, X, ldx, ncta, 0);
     CK(cudaGetLastError());
     CK(cudaEventRecord(b));
     CK(cudaEventSynchronize(b));
@@ -67,8 +67,9 @@ static void sweep(const Layer &L, const char *dt, int reps, int launches) {
     CK(cudaMemcpy(ry, hy.data(), hy.size() * 4, cudaMemcpyHostToDevice));
     CK(cudaMalloc(&X, N * K * 4));
     CK(cudaMalloc(&X0, N * K * 4));
-    NhwcHostGeom g0;
-    nhwc_host_geom(g0, map, (int)sizeof(T), B, P, L.c, L.H, L.H, k, pad, stride, 2);
+    HostGeom g0;
+    const cp_window w{1, k, k, 0, pad, pad, 1, stride, stride, 1, 1, 1};
+    host_geom(g0, map, (int)sizeof(T), B, P, L.c, 1, L.H, L.H, nullptr, w, 2);
     const int ctas[] = {16, 32, 48, 64, 96, 132};
     const int stages[] = {1, 2, 3};
     std::vector<std::vector<float>> t(18);

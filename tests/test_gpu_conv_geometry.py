@@ -252,6 +252,20 @@ def test_window_beyond_the_host_reader_is_refused(engine):
     torch.cuda.synchronize()
 
 
+@pytest.mark.parametrize("dtype", list(_T))
+def test_largest_nhwc_simt_window_equals_unfold(engine, dtype):
+    """kh*kw = 95, the largest window the 2-D entries take on the NHWC SIMT kernel in HBM (kw = 19 is beyond TMA), over
+    c = 140 channels (a full and a partial channel tile), against F.unfold."""
+    win = ((5, 19), (2, 9), 1, 1)
+    H, W, B, nb = 9, 21, 3, 2
+    nchw = _map((nb * B, 140, H, W), dtype, 95, engine.device)
+    rx, ry, P = _points(nb, *_out_size(H, W, win), engine.device)
+    for relu in (False, True):
+        got = _gather(engine, "nhwc_simt", nchw, rx, ry, B, P, win, relu)
+        torch.cuda.synchronize()
+        _assert_same_bits(got.cpu(), _unfold_oracle(nchw, rx, ry, B, win, relu))
+
+
 def test_reference_entries_still_refuse_even_kernels(engine):
     f = torch.zeros(2, 16, 7, 7, device=engine.device)
     rc, err = _raw_gather(engine, f, 16, 7, 7, 0, 2, 2, 0, 0, 1, 1, 1, 1, entry="typed")
