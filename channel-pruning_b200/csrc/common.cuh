@@ -121,6 +121,7 @@ int cp_aux_reserve(cp_handle_t h, size_t bytes, void **out);
 
 static inline size_t cp_align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 static inline int cp_cdiv(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
+static inline bool cp_aligned16(const void *p) { return ((uintptr_t)p & 15) == 0; }
 
 // Carves aligned sub-buffers out of one reservation.
 struct cp_carver {

@@ -18,66 +18,6 @@
 
 namespace {
 
-inline bool al16d(const void *p) { return ((uintptr_t)p & 15) == 0; }
-
-// out[i, j] = alpha * sum_k part[k][i, j] + beta * out[i, j]
-__global__ void reduce_split(const double *__restrict__ part, int64_t split_stride, int nsplit, double *__restrict__ C,
-                             int M, int Nn, int64_t ldc, double alpha, double beta) {
-    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= (int64_t)M * Nn) return;
-    const int i = (int)(e / Nn), j = (int)(e - (int64_t)i * Nn);
-    double s = 0.0;
-    for (int k = 0; k < nsplit; ++k) s += part[(int64_t)k * split_stride + e];
-    double v = alpha * s;
-    if (beta != 0.0) v = fma(beta, C[(int64_t)i * ldc + j], v);
-    C[(int64_t)i * ldc + j] = v;
-}
-
-template <bool A_MC, bool B_NC>
-int gemm_any(cp_handle_t h, const double *A, int64_t lda, const double *B, int64_t ldb, double *C, int64_t ldc, int M, int Nn,
-             int64_t R, double alpha, double beta, cudaStream_t stream) {
-    using namespace cpgemm;
-    Args g{};
-    g.A = A; g.lda = lda; g.B = B; g.ldb = ldb;
-    g.M = M; g.Nn = Nn; g.R = R;
-    g.alpha = alpha; g.beta = beta;
-    g.tile_mode = TILES_ALL;
-    g.a_vec = al16d(A) && (lda % 2 == 0);
-    g.b_vec = al16d(B) && (ldb % 2 == 0);
-    const int tiles = num_tiles(M, Nn, TILES_ALL, BM);
-    const int target = 2 * h->num_sms;
-    int nsplit = 1;
-    if (tiles < target && R >= 8 * BK) {  // tall-skinny products: split the reduction over CTAs
-        nsplit = (target + tiles - 1) / tiles;
-        const int64_t max_by_rows = (R + 4 * BK - 1) / (4 * BK);
-        if (nsplit > max_by_rows) nsplit = (int)max_by_rows;
-        if (nsplit < 1) nsplit = 1;
-    }
-    int64_t rps = (R + nsplit - 1) / nsplit;
-    rps = (rps + BK - 1) / BK * BK;
-    nsplit = (int)((R + rps - 1) / rps);
-    if (nsplit <= 1) {
-        g.nsplit = 1;
-        g.r_per_split = R > 0 ? R : 1;
-        g.C = C; g.ldc = ldc;
-        // fewer 128 x 128 tiles than SMs: 64 x 64 tiles if the cp.async kernel takes the product
-        CP_GEMM_LAUNCH((launch<double, double, A_MC, B_NC>(g, stream, tiles >= h->num_sms ? 128 : 64)));
-        return CP_OK;
-    }
-    void *ws = nullptr;
-    int rc = cp_ws_reserve(h, (size_t)nsplit * M * Nn * sizeof(double), &ws);
-    if (rc) return rc;
-    g.nsplit = nsplit;
-    g.r_per_split = rps;
-    g.C = (double *)ws; g.ldc = Nn; g.c_split_stride = (int64_t)M * Nn;
-    CP_GEMM_LAUNCH((launch<double, double, A_MC, B_NC>(g, stream)));
-    const int64_t total = (int64_t)M * Nn;
-    reduce_split<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>((const double *)ws, g.c_split_stride, nsplit, C, M, Nn, ldc,
-                                                                    alpha, beta);
-    CP_CHECK_LAUNCH();
-    return CP_OK;
-}
-
 // ---------------------------------------------------------------- one-sided Jacobi
 // pair i of step s in the round-robin ("circle") ordering of npad (even) players
 __device__ __forceinline__ void rr_pair(int s, int i, int npad, int &p, int &q) {
@@ -189,17 +129,14 @@ row_norms(double *__restrict__ Ft, int m, int64_t ldf, double *__restrict__ sigm
 }
 
 // ---------------------------------------------------------------- elementwise / column statistics
-// RU = RUraw + b (+ add_mean); U = solve_relu(RU, Z, lambda) (decompose.py:51-59); column sums of U accumulated.
+// RU = RUraw + b (+ add_mean); U = solve_relu(RU, Z, lambda) (decompose.py:51-59).
 __global__ void __launch_bounds__(256)
 solve_relu_kernel(const double *__restrict__ RUraw, int64_t ldr, const double *__restrict__ bias, const double *__restrict__ Z,
-                  int64_t ldz, double lambda, double *__restrict__ U, int64_t ldu, int64_t N, int n,
-                  double *__restrict__ colsum) {
-    // one CTA per 32 columns x 64-row band: coalesced rows, column sums reduced in shared memory then one atomic each
-    __shared__ double part[8][33];
+                  int64_t ldz, double lambda, double *__restrict__ U, int64_t ldu, int64_t N, int n) {
+    // one CTA per 32 columns x 64-row band: coalesced rows
     const int cx = threadIdx.x & 31, rg = threadIdx.x >> 5;
     const int j = blockIdx.x * 32 + cx;
     const int64_t r0 = (int64_t)blockIdx.y * 64;
-    double acc = 0.0;
     if (j < n) {
         const double bj = bias ? bias[j] : 0.0;
         for (int64_t r = r0 + rg; r < r0 + 64 && r < N; r += 8) {
@@ -214,37 +151,7 @@ solve_relu_kernel(const double *__restrict__ RUraw, int64_t ldr, const double *_
             const double cost1 = __dadd_rn(__dmul_rn(d1, d1), __dmul_rn(lambda, __dmul_rn(d2, d2)));
             const double u = (cost0 <= cost1) ? u0 : u1;
             U[r * ldu + j] = u;
-            acc += u;
         }
-    }
-    if (colsum) {
-        part[rg][cx] = acc;
-        __syncthreads();
-        if (rg == 0 && j < n) {
-            double t = 0.0;
-#pragma unroll
-            for (int k = 0; k < 8; ++k) t += part[k][cx];
-            atomicAdd(colsum + j, t);
-        }
-    }
-}
-
-// column sums of an fp64 matrix in a FIXED order (deterministic): CTA = 32 columns, 8 row lanes, serial 8-way add
-__global__ void __launch_bounds__(256)
-colsum_f64(const double *__restrict__ X, int64_t ld, int ncols, int64_t nrows, double scale, double *__restrict__ out) {
-    __shared__ double s1[8][33];
-    const int cx = threadIdx.x & 31, rg = threadIdx.x >> 5;
-    const int col = blockIdx.x * 32 + cx;
-    double a = 0.0;
-    if (col < ncols)
-        for (int64_t r = rg; r < nrows; r += 8) a += X[r * ld + col];
-    s1[rg][cx] = a;
-    __syncthreads();
-    if (rg == 0 && col < ncols) {
-        double t = 0.0;
-#pragma unroll
-        for (int k = 0; k < 8; ++k) t += s1[k][cx];
-        out[col] = t * scale;
     }
 }
 
@@ -267,10 +174,17 @@ extern "C" int cp_gemm_f64(cp_handle_t h, int a_mc, int b_nc, int M, int Nn, int
     CP_REQUIRE(lda >= (a_mc ? M : R) && ldb >= (b_nc ? Nn : R), "cp_gemm_f64: leading dimension too small");
     CP_DEVICE_GUARD(h);
     cudaStream_t stream = (cudaStream_t)stream_;
-    if (a_mc && b_nc) return gemm_any<true, true>(h, A, lda, B, ldb, C, ldc, M, Nn, R, alpha, beta, stream);
-    if (a_mc) return gemm_any<true, false>(h, A, lda, B, ldb, C, ldc, M, Nn, R, alpha, beta, stream);
-    if (b_nc) return gemm_any<false, true>(h, A, lda, B, ldb, C, ldc, M, Nn, R, alpha, beta, stream);
-    return gemm_any<false, false>(h, A, lda, B, ldb, C, ldc, M, Nn, R, alpha, beta, stream);
+    using cpgemm::product;
+    cpgemm::Args g{};
+    g.A = A; g.lda = lda; g.B = B; g.ldb = ldb; g.C = C; g.ldc = ldc;
+    g.M = M; g.Nn = Nn; g.R = R;
+    g.alpha = alpha; g.beta = beta;
+    g.tile_mode = cpgemm::TILES_ALL;
+    const int64_t min_split_r = 8 * cpgemm::BK;  // reductions shorter than 8 stages run unsplit
+    if (a_mc && b_nc) return product<double, double, true, true>(h, g, min_split_r, stream);
+    if (a_mc) return product<double, double, true, false>(h, g, min_split_r, stream);
+    if (b_nc) return product<double, double, false, true>(h, g, min_split_r, stream);
+    return product<double, double, false, false>(h, g, min_split_r, stream);
 }
 
 extern "C" int cp_svd_jacobi(cp_handle_t h, double *Ft, int m, int n, int64_t ldf, double *Wt, int64_t ldw, double *sigma,
@@ -325,11 +239,11 @@ extern "C" int cp_solve_relu(cp_handle_t h, const double *RUraw, int64_t ldr, co
     CP_REQUIRE(N > 0 && n > 0 && ldr >= n && ldz >= n && ldu >= n, "cp_solve_relu: bad shape");
     CP_DEVICE_GUARD(h);
     cudaStream_t stream = (cudaStream_t)stream_;
-    solve_relu_kernel<<<dim3(cp_cdiv(n, 32), cp_cdiv(N, 64)), 256, 0, stream>>>(RUraw, ldr, bias, Z, ldz, lambda, U, ldu, N, n,
-                                                                                 nullptr);
+    solve_relu_kernel<<<dim3(cp_cdiv(n, 32), cp_cdiv(N, 64)), 256, 0, stream>>>(RUraw, ldr, bias, Z, ldz, lambda, U, ldu, N, n);
     CP_CHECK_LAUNCH();
-    if (colmean_out) {  // fixed-order column means (the atomic variant above would not be reproducible)
-        colsum_f64<<<cp_cdiv(n, 32), 256, 0, stream>>>(U, ldu, n, N, 1.0 / (double)N, colmean_out);
+    if (colmean_out) {  // fixed-order column means
+        cpgemm::colsum_kernel<double><<<cp_cdiv(n, 32), 256, 0, stream>>>(U, ldu, n, nullptr, N, nullptr, 1.0 / (double)N,
+                                                                          colmean_out, nullptr);
         CP_CHECK_LAUNCH();
     }
     return CP_OK;
@@ -341,7 +255,7 @@ extern "C" int cp_colstats_f64(cp_handle_t h, const double *X, int64_t ldx, int6
     CP_REQUIRE(N > 0 && n > 0 && ldx >= n, "cp_colstats_f64: bad shape");
     CP_DEVICE_GUARD(h);
     cudaStream_t stream = (cudaStream_t)stream_;
-    colsum_f64<<<cp_cdiv(n, 32), 256, 0, stream>>>(X, ldx, n, N, scale, colsum_out);
+    cpgemm::colsum_kernel<double><<<cp_cdiv(n, 32), 256, 0, stream>>>(X, ldx, n, nullptr, N, nullptr, scale, colsum_out, nullptr);
     CP_CHECK_LAUNCH();
     if (centred_out) {  // centred_out = X - colsum_out (meaningful with scale = 1/N: the column means)
         CP_REQUIRE(ldo >= n, "cp_colstats_f64: ldo < n");

@@ -25,6 +25,7 @@
 //   operand).  Requires 16-byte aligned operands and even leading dimensions (aligned()).
 //
 // launch() takes the async kernel whenever the operands allow it, the register-staged one otherwise.  Bound: FP64 pipe.
+// product() puts launch() behind the split-reduction policy of cp_gram's fp64 products and of cp_gemm_f64.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -489,8 +490,7 @@ __global__ void __launch_bounds__(NT, T == 128 ? 1 : 2) gemm_async_kernel(const 
 // ---------------------------------------------------------------- launches
 // the cp.async copies need 16-byte aligned operands and rows of whole 16-byte chunks
 inline bool aligned(const AsyncArgs &g) {
-    return ((reinterpret_cast<uintptr_t>(g.A) & 15) == 0) && ((reinterpret_cast<uintptr_t>(g.B) & 15) == 0) &&
-           (g.lda % 2 == 0) && (g.ldb % 2 == 0);
+    return cp_aligned16(g.A) && cp_aligned16(g.B) && (g.lda % 2 == 0) && (g.ldb % 2 == 0);
 }
 
 template <int T, bool B_NC>
@@ -535,6 +535,125 @@ inline cudaError_t launch(const Args &g, cudaStream_t stream, int tile = 128) {
     if (grid.x == 0) return cudaSuccess;
     kern<<<grid, NT, SMEM_BYTES, stream>>>(g);
     return cudaGetLastError();
+}
+
+// ---------------------------------------------------------------- products on the handle
+// C[i, j] = alpha * (sum of the nsplit M x Nn partials, in split order) + beta * C[i, j]; C is not read when beta == 0.
+// SYM: upper tiles only, the lower ones come from mirror_upper_tiles.
+template <bool SYM>
+__global__ void reduce_splits(const double *__restrict__ part, int nsplit, double *__restrict__ C, int M, int Nn,
+                              int64_t ldc, double alpha, double beta) {
+    const int64_t total = (int64_t)M * Nn;
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= total) return;
+    const int i = (int)(e / Nn), j = (int)(e - (int64_t)i * Nn);
+    if (SYM && (i / BM) > (j / BN)) return;
+    double s = 0.0;
+    for (int k = 0; k < nsplit; ++k) s += part[k * total + e];
+    double v = alpha * s;
+    if (beta != 0.0) v = fma(beta, C[(int64_t)i * ldc + j], v);
+    C[(int64_t)i * ldc + j] = v;
+}
+
+// C[j, i] = C[i, j] for every element of the strictly-upper T x T tiles, through a padded shared-memory tile so that
+// both the reads and the writes are coalesced.
+template <int T>
+__global__ void __launch_bounds__(256)
+mirror_upper_tiles(double *__restrict__ C, int M, int64_t ldc) {
+    __shared__ double t[32][33];
+    const int bx = blockIdx.x, by = blockIdx.y;  // 32x32 sub-tile (row block by, column block bx)
+    if ((by * 32) / T >= (bx * 32) / T) return;  // only strictly-upper T-tiles
+    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+    for (int r = ty; r < 32; r += 8) {
+        const int i = by * 32 + r, j = bx * 32 + tx;
+        if (i < M && j < M) t[r][tx] = C[(int64_t)i * ldc + j];
+    }
+    __syncthreads();
+    for (int r = ty; r < 32; r += 8) {
+        const int j = bx * 32 + r, i = by * 32 + tx;
+        if (i < M && j < M) C[(int64_t)j * ldc + i] = t[tx][r];
+    }
+}
+
+// C = alpha a b' + beta C, for the operands, shape, row gather, bias, alpha, beta, tile set, C and ldc set in g.
+// Products whose tiles do not fill 2 x SMs, over at least min_split_r reduction rows, split the reduction over CTAs
+// (at least 64 rows per split, a multiple of BK) into fp64 partials in the handle's scratch, summed in a fixed order
+// (deterministic, no atomics).  TILES_UPPER_SYM fills the lower tiles from the upper ones.  R = 0 gives C = beta C.
+template <typename TA, typename TB, bool A_MC, bool B_NC>
+int product(cp_handle_t h, Args g, int64_t min_split_r, cudaStream_t stream) {
+    g.a_vec = cp_aligned16(g.A) && (g.lda % (16 / sizeof(TA)) == 0);
+    g.b_vec = cp_aligned16(g.B) && (g.ldb % (16 / sizeof(TB)) == 0);
+    const int tiles = num_tiles(g.M, g.Nn, g.tile_mode, BM);
+    const int target = 2 * h->num_sms;
+    int nsplit = 1;
+    int64_t rps = g.R;
+    if (tiles < target && g.R > 0 && g.R >= min_split_r) {
+        nsplit = (target + tiles - 1) / tiles;
+        const int64_t max_by_rows = (g.R + 4 * BK - 1) / (4 * BK);
+        if (nsplit > max_by_rows) nsplit = (int)max_by_rows;
+        rps = (g.R + nsplit - 1) / nsplit;
+        rps = (rps + BK - 1) / BK * BK;
+        nsplit = (int)((g.R + rps - 1) / rps);
+    }
+    double *const C = g.C;
+    const int64_t ldc = g.ldc;
+    const bool sym = g.tile_mode == TILES_UPPER_SYM;
+    if (nsplit == 1) {
+        g.nsplit = 1;
+        g.r_per_split = g.R;
+        // fewer 128 x 128 tiles than SMs: 64 x 64 tiles if the cp.async kernel takes the product
+        CP_GEMM_LAUNCH((launch<TA, TB, A_MC, B_NC>(g, stream, tiles >= h->num_sms ? 128 : 64)));
+    } else {
+        void *ws = nullptr;
+        int rc = cp_ws_reserve(h, (size_t)nsplit * g.M * g.Nn * sizeof(double), &ws);
+        if (rc) return rc;
+        g.nsplit = nsplit;
+        g.r_per_split = rps;
+        g.C = (double *)ws; g.ldc = g.Nn; g.c_split_stride = (int64_t)g.M * g.Nn;
+        CP_GEMM_LAUNCH((launch<TA, TB, A_MC, B_NC>(g, stream)));
+        const unsigned blocks = (unsigned)cp_cdiv((int64_t)g.M * g.Nn, 256);
+        if (sym) reduce_splits<true><<<blocks, 256, 0, stream>>>(g.C, nsplit, C, g.M, g.Nn, ldc, g.alpha, g.beta);
+        else reduce_splits<false><<<blocks, 256, 0, stream>>>(g.C, nsplit, C, g.M, g.Nn, ldc, g.alpha, g.beta);
+        CP_CHECK_LAUNCH();
+    }
+    if (sym && g.M > BM) {
+        const int nb32 = (g.M + 31) / 32;
+        mirror_upper_tiles<BM><<<dim3(nb32, nb32), 256, 0, stream>>>(C, g.M, ldc);
+        CP_CHECK_LAUNCH();
+    }
+    return CP_OK;
+}
+
+// scale * column sums (and optionally scale * sums of squares) of X[rows] - bias, fp64 accumulation in a fixed
+// summation order: each CTA owns 32 columns, 8 row lanes, then a serial 8-way add.
+template <typename T>
+__global__ void __launch_bounds__(256)
+colsum_kernel(const T *__restrict__ X, int64_t ld, int ncols, const int32_t *__restrict__ rows, int64_t nrows,
+              const float *__restrict__ bias, double scale, double *__restrict__ sum_out,
+              double *__restrict__ sumsq_out) {
+    __shared__ double s1[8][33], s2[8][33];
+    const int cx = threadIdx.x & 31, rg = threadIdx.x >> 5;
+    const int col = blockIdx.x * 32 + cx;
+    double a = 0.0, q = 0.0;
+    if (col < ncols) {
+        const double b = bias ? (double)bias[col] : 0.0;
+        for (int64_t r = rg; r < nrows; r += 8) {
+            const int64_t row = rows ? (int64_t)rows[r] : r;
+            const double v = (double)__ldg(X + row * ld + col) - b;
+            a += v;
+            q = fma(v, v, q);
+        }
+    }
+    s1[rg][cx] = a;
+    s2[rg][cx] = q;
+    __syncthreads();
+    if (rg == 0 && col < ncols) {
+        double ta = 0.0, tq = 0.0;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) { ta += s1[k][cx]; tq += s2[k][cx]; }
+        if (sum_out) sum_out[col] = ta * scale;
+        if (sumsq_out) sumsq_out[col] = tq * scale;
+    }
 }
 
 }  // namespace cpgemm

@@ -430,8 +430,6 @@ ls_output(const double *__restrict__ Wt, int64_t ld, const double *__restrict__ 
     }
 }
 
-inline bool al16(const void *p) { return ((uintptr_t)p & 15) == 0; }
-
 // C = alpha * a b' + beta C on the solver's fp64 operands:  a(m, r) = A[m * lda + r],
 // b(nn, r) = B_NC ? B[r * ldb + nn] : B[nn * ldb + r].
 // tc: the product may take the tensor cores.  With the handle's tensor-core mode on, products wide enough to fill the
@@ -946,8 +944,8 @@ extern "C" int cp_ls_residual(cp_handle_t h, const float *X, int64_t N, int K, i
     g.nsplit = nsplit > 1 ? nsplit : 1;
     g.r_per_split = nsplit > 1 ? rps : K;
     g.alpha = 1.0; g.beta = 0.0; g.tile_mode = TILES_ALL;
-    g.a_vec = al16(X) && (ldx % 4 == 0);
-    g.b_vec = al16(Wf) && (ldw % 2 == 0);
+    g.a_vec = cp_aligned16(X) && (ldx % 4 == 0);
+    g.b_vec = cp_aligned16(Wf) && (ldw % 2 == 0);
     CP_GEMM_LAUNCH((launch<float, double, false, false>(g, stream)));
     const int64_t count = N * (int64_t)n;
     const unsigned nblk = (unsigned)((count + 255) / 256);

@@ -335,6 +335,7 @@ int cp_gemm_tc_split(cp_handle_t h, int M, int Nn, int R, double alpha, const do
  *   a(m, r)  = a_mc ? A[r * lda + m] : A[m * lda + r]
  *   b(nn, r) = b_nc ? B[r * ldb + nn] : B[nn * ldb + r]
  * Tall-skinny shapes (long reduction, few output tiles) are split over CTAs and summed in a fixed order.
+ * R = 0 gives C = beta * C (A and B are not read).
  */
 int cp_gemm_f64(cp_handle_t h, int a_mc, int b_nc, int M, int Nn, int64_t R, double alpha, const double *A,
                 int64_t lda, const double *B, int64_t ldb, double beta, double *C, int64_t ldc, cp_stream_t stream);

@@ -41,6 +41,20 @@ def test_gemm_f64_all_layouts(engine, M, Nn, R):
     np.testing.assert_allclose(out.cpu().numpy(), -2.0 * want + 0.5 * C0, atol=3 * tol)
 
 
+@pytest.mark.parametrize("a_mc,b_nc", [(0, 0), (0, 1), (1, 0), (1, 1)])
+def test_gemm_f64_empty_reduction_scales_c(engine, a_mc, b_nc):
+    # through the C ABI: Engine.gemm passes an empty operand as NULL, which cp_gemm_f64 refuses
+    M, Nn = 130, 70
+    C0 = np.random.RandomState(4).standard_normal((M, Nn))
+    A = torch.full((M, M), float("nan"), dtype=torch.float64, device=engine.device)  # never read at R = 0
+    B = torch.full((Nn, Nn), float("nan"), dtype=torch.float64, device=engine.device)
+    out = _dev(C0, engine)
+    engine._call(engine.lib.cp_gemm_f64(engine.h, a_mc, b_nc, M, Nn, 0, -2.0, engine._p(A, "const double*"), M,
+                                        engine._p(B, "const double*"), Nn, 0.5, engine._p(out, "double*"), Nn,
+                                        engine._s()))
+    assert np.array_equal(out.cpu().numpy(), 0.5 * C0)
+
+
 @pytest.mark.parametrize("m,n,kind", [(36, 60, "full"), (60, 36, "full"), (200, 200, "full"), (128, 128, "lowrank"),
                                       (768, 300, "decay"), (257, 255, "full")])
 def test_svd_jacobi_matches_lapack(engine, m, n, kind):
