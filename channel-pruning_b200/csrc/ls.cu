@@ -104,6 +104,10 @@ __device__ __forceinline__ void potrf32_warp(double *As, int k0, const double *t
 #pragma unroll
     for (int k = 0; k < SB; ++k) {
         const double tk = __shfl_sync(0xffffffffu, thr, k);
+        if (lane == k) {  // the pivot as met, before a failed one is replaced: a NaN or negative pivot counts as 0
+            const double i0 = inv0_s[k0 + k];
+            if (i0 >= 0.0) ratio_min = fmin(ratio_min, dk > 0.0 ? dk * i0 : 0.0);
+        }
         // pivot must stay above 1e-12 of the original diagonal entry: the squared form of the
         // sigma < 1e-6 sigma_max cut-off LinearRegression applies (sklearn _base.py:752-753, cond=tol=1e-6)
         if (!(dk > tk)) {
@@ -115,8 +119,6 @@ __device__ __forceinline__ void potrf32_warp(double *As, int k0, const double *t
         if (lane == k) {
             l = dk * rs;
             myrs = rs;
-            const double i0 = inv0_s[k0 + k];
-            if (i0 > 0.0) ratio_min = fmin(ratio_min, dk * i0);
         }
         a[k] = l;
         if (k + 1 < SB) {
@@ -232,7 +234,7 @@ potrf128(const double *__restrict__ A, int64_t lda, int nb, double *__restrict__
     double *Tt = Xdt + NSB * SB * LDX_S;          // [3][32][33] temporaries of the block inversion (transposed)
     double *rinv = Tt + 3 * SB * LDX_S;           // [128] 1 / L[k][k]
     double *thr = rinv + PB;                      // [128] pivot thresholds
-    double *inv0 = thr + PB;                      // [128] 1 / original diagonal
+    double *inv0 = thr + PB;                      // [128] 1 / original diagonal (0: not positive; -1: padding)
     double *cb = inv0 + PB;                       // [2][32] column of the pivot step, published to the whole warp
     __shared__ MmTask tasks[3];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -251,7 +253,7 @@ potrf128(const double *__restrict__ A, int64_t lda, int nb, double *__restrict__
     if (tid < PB) {
         const double d0 = tid < nb ? diag0[j0 + tid] : 0.0;
         thr[tid] = tid < nb ? 1e-12 * d0 : 0.0;
-        inv0[tid] = d0 > 0.0 ? 1.0 / d0 : 0.0;
+        inv0[tid] = tid >= nb ? -1.0 : (d0 > 0.0 ? 1.0 / d0 : 0.0);  // an all-zero column meets the ratio 0
     }
     __syncthreads();
 
@@ -505,8 +507,10 @@ static int merge_inverse(cp_handle_t h, double *X, const double *L21, int64_t ld
 // same size.  The substitutions then take ceil(Kd/512) steps instead of ceil(Kd/128).
 // Status: info receives the first failed pivot (1-based, 0: none), ratio the smallest pivot / original diagonal ratio,
 // copied to stat_out (when not NULL) once the factorisation is complete.
-static int chol_factor(cp_handle_t h, double *M, double *L, int64_t ld, int Kd, int nrhs, double *Xinv, double *Tm,
-                       const double *diag0, int32_t *info, double *ratio, double *stat_out, cudaStream_t stream) {
+// tc: the pair updates (near, near2, rest) may take the tensor cores (not in the dual path, whatever the handle's mode).
+static int chol_factor(cp_handle_t h, bool tc, double *M, double *L, int64_t ld, int Kd, int nrhs, double *Xinv,
+                       double *Tm, const double *diag0, int32_t *info, double *ratio, double *stat_out,
+                       cudaStream_t stream) {
     using namespace cpgemm;
     const int Ktot = Kd + nrhs;
     int rc = ensure_side(h, stream);
@@ -587,7 +591,7 @@ static int chol_factor(cp_handle_t h, double *M, double *L, int64_t ld, int Kd, 
         if (!odd) {
             const int w3 = Kd - j2 < PB ? Kd - j2 : PB;
             const double *Pf = L + (int64_t)j2 * ld + j0;
-            rc = dgemm<false>(h, true, 128, TILES_LOWER, 0, Pf, ld, Pf, ld, M + (int64_t)j2 * ld + j2, ld, Ktot - j2, w3, nb,
+            rc = dgemm<false>(h, tc, 128, TILES_LOWER, 0, Pf, ld, Pf, ld, M + (int64_t)j2 * ld + j2, ld, Ktot - j2, w3, nb,
                               -1.0, 1.0, h->side);
             if (rc) return rc;
             CP_CUDA(cudaEventRecord(h->ev_side, h->side));
@@ -597,7 +601,7 @@ static int chol_factor(cp_handle_t h, double *M, double *L, int64_t ld, int Kd, 
             const int je = j0 - PB, R2 = PB + nb;
             const int wn = Kd - j2 < 2 * PB ? Kd - j2 : 2 * PB;  // near: the next pair's two block columns
             const double *Pq = L + (int64_t)j2 * ld + je;
-            rc = dgemm<false>(h, true, 128, TILES_LOWER, 0, Pq, ld, Pq, ld, M + (int64_t)j2 * ld + j2, ld, Ktot - j2, wn, R2,
+            rc = dgemm<false>(h, tc, 128, TILES_LOWER, 0, Pq, ld, Pq, ld, M + (int64_t)j2 * ld + j2, ld, Ktot - j2, wn, R2,
                               -1.0, 1.0, h->side);
             if (rc) return rc;
             CP_CUDA(cudaEventRecord(h->ev_side, h->side));
@@ -610,7 +614,7 @@ static int chol_factor(cp_handle_t h, double *M, double *L, int64_t ld, int Kd, 
                 }
                 const int wm = Kd - j4 < 2 * PB ? Kd - j4 : 2 * PB;
                 const double *P4 = L + (int64_t)j4 * ld + je;
-                rc = dgemm<false>(h, true, 128, TILES_LOWER, 0, P4, ld, P4, ld, M + (int64_t)j4 * ld + j4, ld, Ktot - j4, wm,
+                rc = dgemm<false>(h, tc, 128, TILES_LOWER, 0, P4, ld, P4, ld, M + (int64_t)j4 * ld + j4, ld, Ktot - j4, wm,
                                   R2, -1.0, 1.0, h->side);
                 if (rc) return rc;
                 const int j6 = j4 + wm;
@@ -619,7 +623,7 @@ static int chol_factor(cp_handle_t h, double *M, double *L, int64_t ld, int Kd, 
                     // or the chain's small kernels queue behind them: two thirds of the SMs
                     CP_CUDA(cudaStreamWaitEvent(h->bulk, h->ev_panel, 0));
                     const double *Pr = L + (int64_t)j6 * ld + je;
-                    rc = dgemm<false>(h, true, 128, TILES_LOWER, h->num_sms * 2 / 3, Pr, ld, Pr, ld, M + (int64_t)j6 * ld + j6,
+                    rc = dgemm<false>(h, tc, 128, TILES_LOWER, h->num_sms * 2 / 3, Pr, ld, Pr, ld, M + (int64_t)j6 * ld + j6,
                                       ld, Ktot - j6, Kd - j6, R2, -1.0, 1.0, h->bulk);
                     if (rc) return rc;
                     CP_CUDA(cudaEventRecord(h->ev_bulk, h->bulk));
@@ -734,7 +738,7 @@ static int factor_and_keep(cp_handle_t h, const double *G, const double *Bxy, co
     ls_assemble<<<dim3(cp_cdiv(Ksel, 256), Ksel + n), 256, 0, stream>>>(G, Bxy, sx, sy, 1.0 / (double)N, K, n, sel_cols,
                                                                        Ksel, M, ld, diag0);
     CP_CHECK_LAUNCH();
-    rc = chol_factor(h, M, fac->L, ld, Ksel, n, fac->Linv, fac->Tm, diag0, info_out, fac->ratio, stat_out, stream);
+    rc = chol_factor(h, true, M, fac->L, ld, Ksel, n, fac->Linv, fac->Tm, diag0, info_out, fac->ratio, stat_out, stream);
     if (rc) return rc;
     h->fac.K = Ksel;
     h->fac.Kfull = K;
@@ -1070,7 +1074,7 @@ extern "C" int cp_ls_solve_dual(cp_handle_t h, const float *X, int64_t N, int K,
     else
         dual_rhs<double><<<dim3(cp_cdiv(Ni, 256), n), 256, 0, stream>>>((const double *)Yraw, ldy, y_bias, ymean, N, n, M, ldm);
     CP_CHECK_LAUNCH();
-    rc = chol_factor(h, M, L, ldm, Ni, n, Linv, Tm, diag0, info_out, ratio, stat_out, stream);
+    rc = chol_factor(h, false, M, L, ldm, Ni, n, Linv, Tm, diag0, info_out, ratio, stat_out, stream);
     if (rc) return rc;
     rc = chol_backward(h, false, L, ldm, Ni, Linv, L + (int64_t)Ni * ldm, ldm, At, ldm, n, stream);
     if (rc) return rc;

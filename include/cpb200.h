@@ -80,7 +80,7 @@ int cp_gram_profile(cp_handle_t h, int enable);
  * trailing updates and forward substitutions with >= 256 columns run on the tensor cores in 22-bit split precision
  * (csrc/gemm_tc.cu) -- meant for statistics that came from cp_gram's tensor-core mode and are followed by a
  * refinement step (cp_ls_residual + cp_ls_resolve); the panel factorisations, the panel solves and the pivot-ratio
- * statistic stay fp64. */
+ * statistic stay fp64.  cp_ls_solve_dual is always fp64, whatever this mode. */
 int cp_ls_tensor_cores(cp_handle_t h, int enable);
 int cp_gram_kernel_ms(cp_handle_t h, float *ms);
 
@@ -270,7 +270,8 @@ int cp_lasso_cd_dataform(cp_handle_t h, const float *Z, int64_t ldz, const doubl
  * b_out : n fp64.  info_out : 1 int32 (0 ok, j>0: pivot j fell below 1e-12 of its original diagonal entry --
  * the squared form of the sigma < 1e-6 sigma_max cut-off of LinearRegression, sklearn _base.py:752-753).
  * stat_out : NULL or 1 double: the smallest pivot / original-diagonal ratio met (1 - R^2 of the most collinear
- * column given its predecessors) -- the caller's conditioning signal for choosing the Gram arithmetic.
+ * column given its predecessors) -- the caller's conditioning signal for choosing the Gram arithmetic.  A failed
+ * pivot enters with its own ratio (<= 1e-12; a NaN or non-positive pivot, or an all-zero column, as 1e-300).
  * Requires N - 1 >= Ksel (otherwise use cp_ls_solve_dual).
  */
 int cp_ls_solve(cp_handle_t h, const double *G, const double *Bxy, const double *sx, const double *sy,
