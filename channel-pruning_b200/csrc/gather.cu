@@ -158,6 +158,8 @@ bool cp_gather_tma_applies(const cp_patch_args &a);
 int cp_patch_gather_tma(cp_handle_t h, const cp_patch_args &a);
 // gather_host.cu: the in-place reader of channels-last maps in pinned host memory
 int cp_patch_gather_host(const cp_patch_args &a);
+// gather_tr.cu: the gathers of transposed convolutions, every layout, from HBM or (host_src) pinned host memory
+int cp_patch_gather_tr(const cp_patch_args &a, bool host_src);
 
 template <typename T>
 static void launch_patch_gather_simt(const cp_patch_args &a, bool host_src) {
@@ -194,12 +196,16 @@ struct cp_gather_limits {
     int max_simt_taps;   // channels-last SIMT kernel in HBM; 0: no bound of its own
     int max_host_taps;   // channels-last reader of pinned host maps
     bool refuse_empty;   // refuse a window that leaves the output map empty
+    bool transposed;     // a transposed convolution's window (gather_tr.cu): every tap is range-checked
 };
 // The 2-D entries keep the bounds of their square-window origins: the SIMT tile of 128 channels in 48 KB (95 taps)
 // and the host reader's k <= 9.  Its channel chunks, and the adaptive SIMT tile, would fit larger windows.
 static const cp_gather_limits CP_GATHER_2D = {"cp_patch_gather", false, 95, 81, false};
 // The 3-D entry: the host reader up to 7 x 7 x 7 (a 3 x 7 x 7 stem is 147)
 static const cp_gather_limits CP_GATHER_3D = {"cp_patch_gather_conv3d", true, 0, 343, true};
+// The transposed entries: no bound of a path's own, and no empty output map (output_padding only sets its size)
+static const cp_gather_limits CP_GATHER_TR_2D = {"cp_patch_gather_conv_transpose", false, 0, 0, false, true};
+static const cp_gather_limits CP_GATHER_TR_3D = {"cp_patch_gather_conv_transpose3d", true, 0, 0, false, true};
 
 // Per-axis values as the entry prints them: "h<sep>w" (2-D) or "t<sep>h<sep>w" (3-D)
 static const char *cp_axes(char (&buf)[64], bool d3, const char *sep, int t, int h, int w) {
@@ -252,6 +258,7 @@ static int cp_patch_gather_any(const cp_gather_limits &L, cp_handle_t h, const c
     char s[64];
     // map in (pinned, UVA-mapped) host memory?  then the kernel is a PCIe reader: keep its footprint small
     const cp_mem_kind kind = cp_pointer_kind(a.fmap);
+    if (L.transposed) return cp_patch_gather_tr(a, kind == CP_MEM_HOST);
     if (a.layout == CP_LAYOUT_NHWC) {
         // channels-last map in HBM: whole windows by TMA, rows out by bulk store (gather_tma.cu)
         if (kind == CP_MEM_DEVICE && cp_gather_tma_applies(a)) return cp_patch_gather_tma(h, a);
@@ -303,6 +310,29 @@ extern "C" int cp_patch_gather_conv3d(cp_handle_t h, const void *fmap, int fmap_
     const cp_window g{kt, kh, kw, pad_t, pad_h, pad_w, stride_t, stride_h, stride_w, dil_t, dil_h, dil_w};
     return cp_patch_gather_any(CP_GATHER_3D, h,
                                {CP_GATHER_3D.name, fmap, fmap_dtype, layout, nbatch, B, c, D, H, W, P, randt, randx,
+                                randy, g, relu, X_out, ldx, (cudaStream_t)stream});
+}
+
+extern "C" int cp_patch_gather_conv_transpose(cp_handle_t h, const void *fmap, int fmap_dtype, int nbatch, int B,
+                                              int c, int H, int W, int layout, const int32_t *randx,
+                                              const int32_t *randy, int P, int kh, int kw, int pad_h, int pad_w,
+                                              int stride_h, int stride_w, int dil_h, int dil_w, int relu,
+                                              float *X_out, int64_t ldx, cp_stream_t stream) {
+    const cp_window g{1, kh, kw, 0, pad_h, pad_w, 1, stride_h, stride_w, 1, dil_h, dil_w};
+    return cp_patch_gather_any(CP_GATHER_TR_2D, h,
+                               {CP_GATHER_TR_2D.name, fmap, fmap_dtype, layout, nbatch, B, c, 1, H, W, P, nullptr,
+                                randx, randy, g, relu, X_out, ldx, (cudaStream_t)stream});
+}
+
+extern "C" int cp_patch_gather_conv_transpose3d(cp_handle_t h, const void *fmap, int fmap_dtype, int nbatch, int B,
+                                                int c, int D, int H, int W, int layout, const int32_t *randt,
+                                                const int32_t *randx, const int32_t *randy, int P, int kt, int kh,
+                                                int kw, int pad_t, int pad_h, int pad_w, int stride_t, int stride_h,
+                                                int stride_w, int dil_t, int dil_h, int dil_w, int relu, float *X_out,
+                                                int64_t ldx, cp_stream_t stream) {
+    const cp_window g{kt, kh, kw, pad_t, pad_h, pad_w, stride_t, stride_h, stride_w, dil_t, dil_h, dil_w};
+    return cp_patch_gather_any(CP_GATHER_TR_3D, h,
+                               {CP_GATHER_TR_3D.name, fmap, fmap_dtype, layout, nbatch, B, c, D, H, W, P, randt, randx,
                                 randy, g, relu, X_out, ldx, (cudaStream_t)stream});
 }
 

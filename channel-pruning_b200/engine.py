@@ -258,16 +258,22 @@ class Engine:
         return torch.empty(*shape, dtype=dtype, device=self.device)
 
     # ------------------------------------------------------------------ kernels
-    def patch_gather(self, fmap, randx, randy, B, P, k, pad, stride, relu=True, layout="nchw", out=None, dilation=1):
+    def patch_gather(self, fmap, randx, randy, B, P, k, pad, stride, relu=True, layout="nchw", out=None, dilation=1,
+                     transposed=False):
         """fmap: (nbatch*B, c, H, W) [nchw] or (nbatch*B, H, W, c) [nhwc], float32 / bfloat16 / float16, on device
         or in pinned host memory (read in place over PCIe); randx/randy: (nbatch, P) int32 on device.  Returns X (nbatch*P*B, c*kh*kw)
         fp32 -- 16-bit maps are widened exactly, so X equals the X of fmap.float().
         k, pad, stride, dilation: an int or an (h, w) pair, with the meaning of torch.nn.Conv2d's arguments (pad: the
         top / left padding; the sampled points already respect the output size).  Columns are in F.unfold's order.
-        All ints with dilation 1 is the reference's window, which must be odd (an even square kernel is (k, k))."""
+        All ints with dilation 1 is the reference's window, which must be odd (an even square kernel is (k, k)).
+        transposed: the window of torch.nn.ConvTranspose2d (k, pad = padding, stride, dilation as it takes them; fmap
+        its input map, the points in its output map; cp_patch_gather_conv_transpose).  Then X @
+        weight.transpose(0, 1).reshape(n, -1).T is the layer's output at the points, minus its bias."""
         geo = _gather_map(fmap, B, layout, False)
         (kh, kw), (ph, pw), (sh, sw), (dh, dw) = (conv_pair(v) for v in (k, pad, stride, dilation))
-        if all(isinstance(v, (int, np.integer)) for v in (k, pad, stride, dilation)) and dilation == 1:
+        if transposed:
+            fn, window = self.lib.cp_patch_gather_conv_transpose, (kh, kw, ph, pw, sh, sw, dh, dw)
+        elif all(isinstance(v, (int, np.integer)) for v in (k, pad, stride, dilation)) and dilation == 1:
             fn, window = self.lib.cp_patch_gather_typed, (kh, ph, sh)
         else:
             fn, window = self.lib.cp_patch_gather_conv, (kh, kw, ph, pw, sh, sw, dh, dw)
@@ -279,15 +285,17 @@ class Engine:
         return self._point_gather(self.lib.cp_point_gather_typed, geo, fmap, (randx, randy), B, P, out)
 
     def patch_gather3d(self, fmap, randt, randx, randy, B, P, k, pad, stride, relu=True, layout="ncdhw", out=None,
-                       dilation=1):
+                       dilation=1, transposed=False):
         """fmap: (nbatch*B, c, D, H, W) [ncdhw] or (nbatch*B, D, H, W, c) [ndhwc, channels_last_3d], float32 /
         bfloat16 / float16, on device or in pinned host memory (read in place); randt/randx/randy: (nbatch, P) int32 on
         device, the sampled output points (t, x, y).  Returns X (nbatch*P*B, c*kt*kh*kw) fp32, 16-bit maps widened
         exactly.  k, pad, stride, dilation: an int or a (t, h, w) triple, with the meaning of torch.nn.Conv3d's
-        arguments (pad: the front / top / left padding).  Columns are in Conv3d.weight.reshape(n, -1)'s order."""
+        arguments (pad: the front / top / left padding).  Columns are in Conv3d.weight.reshape(n, -1)'s order.
+        transposed: the window of torch.nn.ConvTranspose3d, as for patch_gather (cp_patch_gather_conv_transpose3d)."""
         geo = _gather_map(fmap, B, layout, True)
         (kt, kh, kw), (pt, ph, pw), (st, sh, sw), (dt, dh, dw) = (conv_triple(v) for v in (k, pad, stride, dilation))
-        return self._patch_gather(self.lib.cp_patch_gather_conv3d, geo, fmap, (randt, randx, randy), B, P,
+        fn = self.lib.cp_patch_gather_conv_transpose3d if transposed else self.lib.cp_patch_gather_conv3d
+        return self._patch_gather(fn, geo, fmap, (randt, randx, randy), B, P,
                                   kt * kh * kw, (kt, kh, kw, pt, ph, pw, st, sh, sw, dt, dh, dw), relu, out)
 
     def point_gather3d(self, fmap, randt, randx, randy, B, P, layout="ncdhw", out=None):

@@ -12,6 +12,7 @@ coupled and this sharding does not apply (use lib.net.Net.R3 on one GPU).
 """
 from __future__ import annotations
 
+import math
 import os
 import time
 
@@ -113,7 +114,8 @@ def prune_layers(eng: Engine, shapes, datas, right0=1e-3, rank_tol=.1, from_host
     or float16, laid out as datas[i]['host_layout']: 'nchw' (default) or 'nhwc') and copied in the pipeline; to_host:
     results are copied back to pinned host memory.
     Conv3d layers (synth.LayerShape3d, whose data carry randt) may stand alone or among 2-D ones; their layouts are
-    'ncdhw' (default) or 'ndhwc'.
+    'ncdhw' (default) or 'ndhwc'.  Transposed layers (shape.transposed: ConvTranspose2d / 3d) are gathered with their
+    own window; W2 and the returned W are (n, c, *window) as for every layer, W.transpose(0, 1) the new weight.
     trace: optional dict; filled with {layer name: [(label, timing event), ...]} plus '_t0' (device timeline
     of the step: profiles/e2e_breakdown.py prints it).
     Batch mode: the problems are INDEPENDENT -- every alpha search starts from ``right0`` and the seeds come with the
@@ -139,6 +141,8 @@ def prune_layers(eng: Engine, shapes, datas, right0=1e-3, rank_tol=.1, from_host
     return [res_o[inv[i]] for i in range(len(shapes))]
 
 
+# Both rates were measured for the conv readers.  The transposed-convolution readers (gather_tr.cu) are charged at
+# them too: their line rates are not measured.
 # read requests per second of the in-place gather over PCIe (profiles/zc_rate.py; H100 80GB HBM3 SXM, PCIe 5)
 ZC_LINES_PER_S = 2.6e8
 # full 128-byte lines per second of the in-place NHWC reader, whose requests are whole lines of contiguous window rows
@@ -182,7 +186,10 @@ def zero_copy_lines(s, esize=4, layout="nchw"):
     Square, undilated windows give the counts the transfer rates ZC_LINES_PER_S and ZC_NHWC_LINES_PER_S were
     measured with.
     Conv3d layers (s.kt): 'ncdhw' counts c*kt*kh rows of kw taps, 'ndhwc' kt*kh runs of kw*c*esize bytes -- kt times
-    the 2-D count of the (kh, kw) window rows of one frame (frames are H*W pixels apart)."""
+    the 2-D count of the (kh, kw) window rows of one frame (frames are H*W pixels apart).
+    Transposed layers (s.transposed): _zero_copy_lines_tr."""
+    if getattr(s, "transposed", False):
+        return _zero_copy_lines_tr(s, esize, layout)
     if _is3d(s):
         flat = _Frame(s)
         return s.kt * zero_copy_lines(flat, esize, "nhwc" if layout in ("nhwc", "ndhwc") else "nchw")
@@ -200,6 +207,36 @@ def zero_copy_lines(s, esize=4, layout="nchw"):
     span = (kh - 1) * dh * row + span_w * esize
     lines = min(kh * per_row, -(-span // 128) + 1) if kh * kw > 1 else 1
     return s.N * s.c * lines
+
+
+def _tr_touched(k, stride, dil):
+    """One axis of a transposed window: the most input coordinates one output coordinate's valid taps read,
+    ceil(k / (stride / g)), and their spacing dil / g (g = gcd(stride, dil)), whatever the output coordinate's phase."""
+    g = math.gcd(stride, dil)
+    return -(-k // (stride // g)), dil // g
+
+
+def _zero_copy_lines_tr(s, esize, layout):
+    """128-byte lines the in-place gather of a transposed layer touches, an upper bound over the phases of the points
+    for a map whose base is 128-byte aligned.  Per point the valid taps read m_t x m_h input rows (_tr_touched; m_t = 1
+    in 2-D) and, in each, m_w pixels sw apart.
+    nchw: per channel and row, the m_w elements span ((m_w - 1) sw + 1) * esize bytes: at most one line more than
+    that span fills, and never more than m_w lines.
+    nhwc: per row, the m_w pixels' c channels span ((m_w - 1) sw + 1) * c * esize bytes (m_w runs of c * esize bytes
+    when sw > 1, if that is fewer), plus one line per run when the pixel stride is not a multiple of 128 bytes."""
+    axes = ([(s.kt, s.stride_t, s.dil_t)] if _is3d(s) else []) + [(s.kh, s.stride_h, s.dil_h),
+                                                                    (s.kw, s.stride_w, s.dil_w)]
+    touched = [_tr_touched(*a) for a in axes]
+    rows = int(np.prod([m for m, _ in touched[:-1]]))
+    mw, sw = touched[-1]
+    span = (mw - 1) * sw + 1  # pixels from the first touched one of a row to its last
+    if layout in ("nhwc", "ndhwc"):
+        tail = 1 if (s.c * esize) % 128 else 0
+        per_row = -(-span * s.c * esize // 128) + tail
+        if sw > 1:
+            per_row = min(per_row, mw * (-(-s.c * esize // 128) + tail))
+        return s.N * rows * per_row
+    return s.N * s.c * rows * min(mw, -(-span * esize // 128) + 1)
 
 
 class _Frame:

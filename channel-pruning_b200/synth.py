@@ -62,16 +62,40 @@ RESNET50 = [
 ]
 
 
+def _out_size(n, k, pad, stride, dil, output_padding, transposed):
+    """One axis of the output map, PyTorch's formula: Conv (n + 2 pad - dil (k - 1) - 1) // stride + 1, ConvTranspose
+    (n - 1) stride - 2 pad + dil (k - 1) + output_padding + 1 with output_padding < max(stride, dil)."""
+    if transposed:
+        assert 0 <= output_padding < max(stride, dil), "output_padding must be smaller than either stride or dilation"
+        out = (n - 1) * stride - 2 * pad + dil * (k - 1) + output_padding + 1
+    else:
+        assert output_padding == 0, "output_padding is an argument of transposed convolutions"
+        out = (n + 2 * pad - dil * (k - 1) - 1) // stride + 1
+    assert out >= 1, "empty output map"
+    return out
+
+
+def _conv_args(s):
+    a = dict(k=s.k, pad=s.pad, stride=s.stride, dilation=s.dilation)
+    if s.transposed:
+        a["transposed"] = True
+    return a
+
+
 class LayerShape:
     """One layer problem: a convolution with c input and n output channels on an H x W input map (W = H unless
     given).  k, pad, stride and dilation are ints or (h, w) pairs, as torch.nn.Conv2d takes them (groups == 1); the
     reference's layers are square, odd and undilated, and for those k, pad and stride keep their plain int meaning.
     kh, kw, pad_h, pad_w, stride_h, stride_w, dil_h, dil_w: the per-axis geometry; k2 = kh*kw taps per channel;
-    Ho x Wo: the output map (PyTorch's formula), the range of the sampled points."""
+    Ho x Wo: the output map (PyTorch's formula), the range of the sampled points.
+    transposed: a torch.nn.ConvTranspose2d consumer (k, pad = padding, stride, dilation and output_padding as it takes
+    them; H x W its input map); W2 is then (n, c, kh, kw) = weight.transpose(0, 1), the orientation of every layer."""
 
-    def __init__(self, name, c, n, H, k=3, pad=1, stride=1, N=5000, B=10, P=10, rank=None, dilation=1, W=None):
+    def __init__(self, name, c, n, H, k=3, pad=1, stride=1, N=5000, B=10, P=10, rank=None, dilation=1, W=None,
+                 transposed=False, output_padding=0):
         self.name, self.c, self.n, self.H, self.W = name, c, n, H, H if W is None else W
         self.k, self.pad, self.stride, self.dilation = k, pad, stride, dilation
+        self.transposed, self.output_padding = bool(transposed), output_padding
         self.kh, self.kw = conv_pair(k)
         self.pad_h, self.pad_w = conv_pair(pad)
         self.stride_h, self.stride_w = conv_pair(stride)
@@ -86,14 +110,13 @@ class LayerShape:
             self.rank = c
         self.K = c * self.k2
         self.S = min(400, N // 20)
-        # output map (torch.nn.Conv2d): (H + 2 pad - dil (k - 1) - 1) // stride + 1 per axis
-        self.Ho = (self.H + 2 * self.pad_h - self.dil_h * (self.kh - 1) - 1) // self.stride_h + 1
-        self.Wo = (self.W + 2 * self.pad_w - self.dil_w * (self.kw - 1) - 1) // self.stride_w + 1
-        assert self.Ho >= 1 and self.Wo >= 1, "empty output map"
+        self.Ho, self.Wo = (_out_size(*a, self.transposed) for a in zip(
+            (self.H, self.W), (self.kh, self.kw), (self.pad_h, self.pad_w), (self.stride_h, self.stride_w),
+            (self.dil_h, self.dil_w), conv_pair(output_padding)))
 
     def conv_args(self):
-        """(k, pad, stride) and dilation as Engine.patch_gather takes them"""
-        return dict(k=self.k, pad=self.pad, stride=self.stride, dilation=self.dilation)
+        """(k, pad, stride), dilation and (for a transposed layer) transposed, as Engine.patch_gather takes them"""
+        return _conv_args(self)
 
     def cost(self):
         """Rough relative cost (Gram + Cholesky flops) for load balancing across GPUs."""
@@ -105,11 +128,14 @@ class LayerShape3d:
     """One layer problem of a Conv3d consumer with c input and n output channels on a D x H x W input map (W = H unless
     given).  k, pad, stride and dilation are ints or (t, h, w) triples, as torch.nn.Conv3d takes them (groups == 1).
     kt, kh, kw, pad_t, ..., dil_w: the per-axis geometry; k2 = kt*kh*kw taps per channel (what the solver sees: X is
-    (N, c*k2)); To x Ho x Wo: the output map (PyTorch's formula), the range of the sampled points (t, x, y)."""
+    (N, c*k2)); To x Ho x Wo: the output map (PyTorch's formula), the range of the sampled points (t, x, y).
+    transposed, output_padding: a torch.nn.ConvTranspose3d consumer, as for LayerShape."""
 
-    def __init__(self, name, c, n, D, H, k=3, pad=1, stride=1, N=5000, B=10, P=10, rank=None, dilation=1, W=None):
+    def __init__(self, name, c, n, D, H, k=3, pad=1, stride=1, N=5000, B=10, P=10, rank=None, dilation=1, W=None,
+                 transposed=False, output_padding=0):
         self.name, self.c, self.n, self.D, self.H, self.W = name, c, n, D, H, H if W is None else W
         self.k, self.pad, self.stride, self.dilation = k, pad, stride, dilation
+        self.transposed, self.output_padding = bool(transposed), output_padding
         self.kt, self.kh, self.kw = conv_triple(k)
         self.pad_t, self.pad_h, self.pad_w = conv_triple(pad)
         self.stride_t, self.stride_h, self.stride_w = conv_triple(stride)
@@ -125,15 +151,15 @@ class LayerShape3d:
             self.rank = c
         self.K = c * self.k2
         self.S = min(400, N // 20)
-        # output map (torch.nn.Conv3d): (in + 2 pad - dil (k - 1) - 1) // stride + 1 per axis
-        self.To = (self.D + 2 * self.pad_t - self.dil_t * (self.kt - 1) - 1) // self.stride_t + 1
-        self.Ho = (self.H + 2 * self.pad_h - self.dil_h * (self.kh - 1) - 1) // self.stride_h + 1
-        self.Wo = (self.W + 2 * self.pad_w - self.dil_w * (self.kw - 1) - 1) // self.stride_w + 1
-        assert self.To >= 1 and self.Ho >= 1 and self.Wo >= 1, "empty output map"
+        self.To, self.Ho, self.Wo = (_out_size(*a, self.transposed) for a in zip(
+            (self.D, self.H, self.W), self.window, (self.pad_t, self.pad_h, self.pad_w),
+            (self.stride_t, self.stride_h, self.stride_w), (self.dil_t, self.dil_h, self.dil_w),
+            conv_triple(output_padding)))
 
     def conv_args(self):
-        """(k, pad, stride) and dilation as Engine.patch_gather3d takes them"""
-        return dict(k=self.k, pad=self.pad, stride=self.stride, dilation=self.dilation)
+        """(k, pad, stride), dilation and (for a transposed layer) transposed, as Engine.patch_gather3d takes them"""
+        return _conv_args(self)
+
 
     def cost(self):
         """Rough relative cost (Gram + Cholesky flops) for load balancing across GPUs."""
@@ -162,6 +188,32 @@ def r3d18_layers(N=5000, B=10, P=50):
     return [LayerShape3d(nm, c, n, D, H, k=3, pad=1, stride=st, N=N, B=B, P=P) for nm, c, n, D, H, st in R3D18]
 
 
+# The transposed convolutions of three decoder families: (name, c_in, n_out, H = W (3-D: D = H = W) of the layer's
+# INPUT map, k, stride, pad), groups == 1.
+# A same-padded 2-D U-Net on 256 x 256 images: the up-convolutions ConvTranspose2d(c, c/2, 2, stride 2).
+UNET_UP = [("up1", 1024, 512, 16, 2, 2, 0), ("up2", 512, 256, 32, 2, 2, 0), ("up3", 256, 128, 64, 2, 2, 0),
+           ("up4", 128, 64, 128, 2, 2, 0)]
+# A 3-D nnU-Net-style decoder on 128^3 patches (features 32 ... 320): ConvTranspose3d(k = stride = 2).
+NNUNET3D_UP = [("tu0", 320, 320, 4, 2, 2, 0), ("tu1", 320, 256, 8, 2, 2, 0), ("tu2", 256, 128, 16, 2, 2, 0),
+               ("tu3", 128, 64, 32, 2, 2, 0), ("tu4", 64, 32, 64, 2, 2, 0)]
+# One DCGAN-style generator layer: ConvTranspose2d(256, 128, 4, stride 2, padding 1), overlapping windows.
+DCGAN_UP = [("dcgan.up3", 256, 128, 16, 4, 2, 1)]
+
+
+def conv_transpose_layers(N=5000):
+    """{network: its transposed-convolution layer problems} of UNET_UP, NNUNET3D_UP and DCGAN_UP.  B and P keep the
+    synthetic fp32 maps within about 10 GB: the 2-D ones at B = 10, P = 50 (100 images, 1.6 GB in all), the 3-D ones at
+    B = 5, P = 100 (50 volumes; 3.4 GB of the 4.3 GB the 64 x 64^3 map of tu4)."""
+    return {
+        "unet2d": [LayerShape(nm, c, n, H, k=k, stride=st, pad=p, N=N, B=10, P=50, transposed=True)
+                   for nm, c, n, H, k, st, p in UNET_UP],
+        "nnunet3d": [LayerShape3d(nm, c, n, H, H, k=k, stride=st, pad=p, N=N, B=5, P=100, transposed=True)
+                     for nm, c, n, H, k, st, p in NNUNET3D_UP],
+        "dcgan": [LayerShape(nm, c, n, H, k=k, stride=st, pad=p, N=N, B=10, P=50, transposed=True)
+                  for nm, c, n, H, k, st, p in DCGAN_UP],
+    }
+
+
 def vgg16_layers(N=5000, B=10, P=10):
     return [LayerShape(nm, c, n, H, N=N, B=B, P=P) for nm, c, n, H in VGG16]
 
@@ -184,7 +236,10 @@ def make_problem_numpy(shape: LayerShape, seed: int, noise=0.01):
     randy = r.randint(0, s.Wo, (s.nbatch, s.P)).astype(np.int32)
     W2 = (r.standard_normal((s.n, s.c, s.kh, s.kw)) * np.sqrt(2.0 / (s.c * s.k2))).astype(np.float32)
     b2 = (0.01 * r.standard_normal(s.n)).astype(np.float32)
-    X = gather_patches_numpy(fmap, randx, randy, s.B, s.k, s.pad, s.stride, relu=True, dilation=s.dilation)
+    if s.transposed:
+        X = gather_patches_tr_numpy(fmap, randx, randy, s.B, s.k, s.pad, s.stride, relu=True, dilation=s.dilation)
+    else:
+        X = gather_patches_numpy(fmap, randx, randy, s.B, s.k, s.pad, s.stride, relu=True, dilation=s.dilation)
     Y = X.reshape(s.N, -1).astype(np.float64) @ W2.reshape(s.n, -1).T.astype(np.float64) + b2
     Y = Y + noise * Y.std() * r.standard_normal(Y.shape)
     feats = Y.astype(np.float32)
@@ -224,7 +279,8 @@ def _make_problem3d_numpy(s, seed, noise):
     randy = r.randint(0, s.Wo, (s.nbatch, s.P)).astype(np.int32)
     W2 = (r.standard_normal((s.n, s.c) + s.window) * np.sqrt(2.0 / (s.c * s.k2))).astype(np.float32)
     b2 = (0.01 * r.standard_normal(s.n)).astype(np.float32)
-    X = gather_patches3d_numpy(fmap, randt, randx, randy, s.B, s.k, s.pad, s.stride, relu=True, dilation=s.dilation)
+    gather = gather_patches_tr3d_numpy if s.transposed else gather_patches3d_numpy
+    X = gather(fmap, randt, randx, randy, s.B, s.k, s.pad, s.stride, relu=True, dilation=s.dilation)
     Y = X.reshape(s.N, -1).astype(np.float64) @ W2.reshape(s.n, -1).T.astype(np.float64) + b2
     Y = Y + noise * Y.std() * r.standard_normal(Y.shape)
     feats = Y.astype(np.float32)
@@ -250,6 +306,50 @@ def gather_patches3d_numpy(fmap, randt, randx, randy, B, k, pad, stride, relu, d
     if relu:
         np.maximum(out, 0, out=out)
     return out
+
+
+def _tr_axis_numpy(x, pad, stride, dil, k, n):
+    """One axis of a transposed window: (input coordinate, valid) of every tap, shape x.shape + (k,).  Tap i of output
+    coordinate x reads (x + pad - dil i) / stride when that division is exact and lands in [0, n)."""
+    num = x[..., None].astype(np.int64) + pad - dil * np.arange(k)
+    ok = (num >= 0) & (num % stride == 0)
+    h = np.where(ok, num // stride, 0)
+    ok &= h < n
+    return np.where(ok, h, 0), ok
+
+
+def gather_patches_tr3d_numpy(fmap, randt, randx, randy, B, k, pad, stride, relu, dilation=1):
+    """The patch gather of torch.nn.ConvTranspose3d in numpy: fmap (nimg, c, D, H, W) is the layer's input map, the
+    points (t, x, y) lie in its output map; rows (batch, point, image), columns (c, kt, kh, kw), zero for invalid taps.
+    k, pad, stride, dilation: ints or (t, h, w) triples."""
+    (kt, kh, kw), (pt, ph, pw), (st, sh, sw), (dt, dh, dw) = (conv_triple(v) for v in (k, pad, stride, dilation))
+    nimg, c, D, H, W = fmap.shape
+    nbatch, P = np.asarray(randx).shape
+    (tt, ot), (hh, oh), (ww, ow) = (_tr_axis_numpy(np.asarray(r), *a) for r, a in (
+        (randt, (pt, st, dt, kt, D)), (randx, (ph, sh, dh, kh, H)), (randy, (pw, sw, dw, kw, W))))
+    img = (np.arange(nbatch)[:, None, None] * B + np.arange(B)[None, None, :])[..., None, None, None, None]
+    a = np.arange(c)[:, None, None, None]
+
+    def ax(v, axis):  # (nbatch, P, k) -> broadcastable against (nbatch, P, B, c, kt, kh, kw) on tap axis 4 + axis
+        shape = [nbatch, P, 1, 1, 1, 1, 1]
+        shape[4 + axis] = v.shape[-1]
+        return v.reshape(shape)
+
+    vals = fmap[img, a, ax(tt, 0), ax(hh, 1), ax(ww, 2)]
+    ok = ax(ot, 0) & ax(oh, 1) & ax(ow, 2)
+    out = np.where(ok, vals, np.zeros((), dtype=fmap.dtype)).reshape(nbatch * P * B, c, kt, kh, kw)
+    if relu:
+        np.maximum(out, 0, out=out)
+    return out
+
+
+def gather_patches_tr_numpy(fmap, randx, randy, B, k, pad, stride, relu, dilation=1):
+    """gather_patches_tr3d_numpy for torch.nn.ConvTranspose2d: the one-frame case, columns (c, kh, kw).  k, pad,
+    stride, dilation: ints or (h, w) pairs."""
+    (kh, kw), (ph, pw), (sh, sw), (dh, dw) = (conv_pair(v) for v in (k, pad, stride, dilation))
+    X = gather_patches_tr3d_numpy(fmap[:, :, None], np.zeros_like(randx), randx, randy, B, (1, kh, kw), (0, ph, pw),
+                                  (1, sh, sw), relu, dilation=(1, dh, dw))
+    return X.reshape(X.shape[0], X.shape[1], kh, kw)
 
 
 def fmap_nchw(d):

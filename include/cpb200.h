@@ -165,6 +165,37 @@ int cp_patch_gather_conv3d(cp_handle_t h, const void *fmap, int fmap_dtype, int 
                            cp_stream_t stream);
 
 /*
+ * Patch gathers for torch.nn.ConvTranspose2d / ConvTranspose3d (groups == 1): the up-convolutions of U-Net and
+ * 3-D U-Net decoders, FCN heads, DCGAN-style generators.
+ *   fmap   : the transposed convolution's INPUT map, nbatch*B images of c x H x W (3-D: c x D x H x W), layout, dtype
+ *            and memory (device or pinned host, read in place) as for cp_patch_gather_conv / _conv3d.
+ *   randx, randy (3-D: randt, randx, randy) : nbatch*P sampled points of its OUTPUT map.
+ *   kh, kw, pad, stride, dil : the arguments of nn.ConvTranspose2d (kernel_size, padding, stride, dilation) per axis.
+ * Output point (x, y) reads, for tap (i, j), the input pixel
+ *     h = (x + pad_h - dil_h*i) / stride_h,   w = (y + pad_w - dil_w*j) / stride_w
+ * when both divisions are exact and 0 <= h < H, 0 <= w < W, otherwise 0 (3-D: the depth axis likewise), into column
+ * a*kh*kw + i*kw + j (3-D: a*kt*kh*kw + (u*kh + i)*kw + j), the conv gathers' order.  So
+ * X_out @ weight.transpose(0, 1).reshape(n, -1).T is the transposed convolution's output at the points, minus its bias.
+ * output_padding only sets the output map's size, which the sampled points already respect: it is no argument.
+ * relu as in cp_patch_gather_conv.  X_out: (nbatch*P*B) x (c*kh*kw) (3-D: c*kt*kh*kw) fp32, leading dimension ldx.
+ * Before any device work, CP_ERR_INVALID with a message for: an unknown dtype or layout, a NULL pointer, a bad shape,
+ * an extent, stride or dilation < 1, a padding < 0, more than 4096 taps, ldx below c*kh*kw (c*kt*kh*kw).  Every tap is
+ * range-checked, so no window is refused for leaving the output map empty.
+ * Paths (csrc/gather_tr.cu), bit-identical: channels first one CTA per output row; channels last per (row, channel
+ * tile) with the touched pixels' channels staged in shared memory; pinned host maps read in place by the same kernels
+ * with a small persistent grid.
+ */
+int cp_patch_gather_conv_transpose(cp_handle_t h, const void *fmap, int fmap_dtype, int nbatch, int B, int c, int H,
+                                   int W, int layout, const int32_t *randx, const int32_t *randy, int P, int kh,
+                                   int kw, int pad_h, int pad_w, int stride_h, int stride_w, int dil_h, int dil_w,
+                                   int relu, float *X_out, int64_t ldx, cp_stream_t stream);
+int cp_patch_gather_conv_transpose3d(cp_handle_t h, const void *fmap, int fmap_dtype, int nbatch, int B, int c, int D,
+                                     int H, int W, int layout, const int32_t *randt, const int32_t *randx,
+                                     const int32_t *randy, int P, int kt, int kh, int kw, int pad_t, int pad_h,
+                                     int pad_w, int stride_t, int stride_h, int stride_w, int dil_t, int dil_h,
+                                     int dil_w, int relu, float *X_out, int64_t ldx, cp_stream_t stream);
+
+/*
  * Point gather -- replaces the gather of Net.extract_features (lib/net.py:509-519):
  *   Y_out[(batch*P+point)*B + image, j] = fmap[batch*B+image, j, randx, randy].
  * fp32 out (the reference widens to fp64; the bias of lib/net.py:1707 is applied
