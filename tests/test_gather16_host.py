@@ -4,6 +4,8 @@ import types
 
 import pytest
 
+import gather_checks as GC
+
 torch = pytest.importorskip("torch")
 
 
@@ -19,19 +21,13 @@ def _maps(shapes, dtype):
     return [dict(fmap_host=torch.empty((s.nbatch * s.B, s.c, s.H, s.W), dtype=dtype, device="meta")) for s in shapes]
 
 
-def _all_shapes():
-    import cpb200
-
-    return cpb200.synth.vgg16_layers() + cpb200.synth.resnet50_layers()
-
-
 def test_fp32_maps_keep_their_plan(monkeypatch):
     """4-byte maps: the same line counts and the same per-layer plan as a map described by numel() alone."""
     from cpb200 import pruner
 
     monkeypatch.delenv("CPB200_DMA_MAX_MB", raising=False)
     monkeypatch.delenv("CPB200_DMA_RATIO", raising=False)
-    shapes = _all_shapes()
+    shapes = GC.all_shapes()
     for s in shapes:
         assert pruner.zero_copy_lines(s) == pruner.zero_copy_lines(s, 4) == _fp32_zero_copy_lines(s)
 

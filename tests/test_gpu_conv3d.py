@@ -9,12 +9,12 @@ import pytest
 
 import conv3d_oracle as C3
 import cp_oracle as O
+import gather_checks as GC
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
 F = pytest.importorskip("torch.nn.functional")
 
-_T = {"fp32": torch.float32, "bf16": torch.bfloat16, "fp16": torch.float16}
 # (kernel_size, padding, stride, dilation), ints or (t, h, w) triples as nn.Conv3d takes them
 WINDOWS = {
     "1x1x1": (1, 0, 1, 1), "3x3x3": (3, 1, 1, 1), "1x3x3": ((1, 3, 3), (0, 1, 1), 1, 1),
@@ -33,47 +33,6 @@ def _tr(v):
 def _out_size(D, H, W, win):
     k, pad, stride, dil = (_tr(v) for v in win)
     return tuple((n + 2 * p - d * (kk - 1) - 1) // s + 1 for n, kk, p, s, d in zip((D, H, W), k, pad, stride, dil))
-
-
-def _map(shape, dtype, seed, device):
-    """N(0,1) drawn in fp32 and rounded to dtype, with -0, +-inf, NaN and subnormals seeded in."""
-    g = torch.Generator(device=device)
-    g.manual_seed(seed)
-    fm = torch.randn(shape, generator=g, device=device)
-    flat = fm.view(-1)
-    specials = torch.tensor([-0.0, float("inf"), float("-inf"), float("nan"), 6e-8, -3e-6, 4e-5, 1e-39, -5e-39,
-                             1e-44], device=device)
-    idx = torch.randperm(flat.numel(), generator=g, device=device)[:max(len(specials), flat.numel() // 40)]
-    flat[idx] = specials[torch.arange(idx.numel(), device=device) % len(specials)]
-    return fm.to(_T[dtype])
-
-
-def _pinned(t):
-    h = torch.empty(t.shape, dtype=t.dtype, pin_memory=True)
-    h.copy_(t)
-    return h
-
-
-def _assert_same_bits(got, want):
-    """Bit equality (so -0 and +0 differ); NaN positions compared separately, their payloads not."""
-    got, want = got.cpu(), want.cpu()
-    assert got.dtype == want.dtype == torch.float32 and got.shape == want.shape
-    ng, nw = torch.isnan(got), torch.isnan(want)
-    assert torch.equal(ng, nw)
-    z = torch.zeros_like(got)
-    assert torch.equal(torch.where(ng, z, got).view(torch.int32), torch.where(nw, z, want).view(torch.int32))
-
-
-def _points(nb, To, Ho, Wo, device):
-    """Every corner of the output volume, border points and the centre, in varying order per batch."""
-    pts = [(t, x, y) for t in (0, To - 1) for x in (0, Ho - 1) for y in (0, Wo - 1)]
-    pts += [(To // 2, Ho // 2, Wo // 2), (0, Ho // 2, Wo - 1), (To - 1, 1 % Ho, Wo // 2), (To // 2, 0, 1 % Wo)]
-    out = []
-    for axis in range(3):
-        v = torch.tensor([[p[axis] for p in pts]] * nb, dtype=torch.int32, device=device)
-        v[1] = v[1].flip(0)
-        out.append(v)
-    return out[0], out[1], out[2], len(pts)
 
 
 def _torch_gather(ncdhw, rt, rx, ry, B, win, relu):
@@ -99,12 +58,12 @@ def _gather(engine, path, ncdhw, rt, rx, ry, B, P, win, relu, out=None):
     layout, host, _ = PATHS[path]
     m = ncdhw if layout == "ncdhw" else ncdhw.permute(0, 2, 3, 4, 1).contiguous()
     if host:
-        m = _pinned(m)
+        m = GC.pinned(m)
     k, pad, stride, dil = win
     return engine.patch_gather3d(m, rt, rx, ry, B, P, k, pad, stride, relu=relu, layout=layout, dilation=dil, out=out)
 
 
-@pytest.mark.parametrize("dtype", list(_T))
+@pytest.mark.parametrize("dtype", list(GC.FMAP_DTYPES))
 @pytest.mark.parametrize("path", list(PATHS))
 @pytest.mark.parametrize("wname", list(WINDOWS))
 def test_gather3d_bits_equal_torch(engine, dtype, path, wname):
@@ -113,12 +72,13 @@ def test_gather3d_bits_equal_torch(engine, dtype, path, wname):
     c = PATHS[path][2]
     D, H, W, B, nb = 5, 9, 8, 3, 2
     To, Ho, Wo = _out_size(D, H, W, win)
-    ncdhw = _map((nb * B, c, D, H, W), dtype, zlib.crc32(("%s/%s/%s" % (wname, path, dtype)).encode()) % 10007, dev)
-    rt, rx, ry, P = _points(nb, To, Ho, Wo, dev)
+    seed = zlib.crc32(("%s/%s/%s" % (wname, path, dtype)).encode()) % 10007
+    ncdhw = GC.special_map((nb * B, c, D, H, W), dtype, seed, dev)
+    rt, rx, ry, P = GC.points3d(nb, To, Ho, Wo, dev)
     for relu in (False, True):
         got = _gather(engine, path, ncdhw, rt, rx, ry, B, P, win, relu)
         torch.cuda.synchronize()
-        _assert_same_bits(got, _torch_gather(ncdhw, rt, rx, ry, B, win, relu))
+        GC.assert_same_bits(got, _torch_gather(ncdhw, rt, rx, ry, B, win, relu))
 
 
 def test_torch_gather_agrees_with_the_numpy_oracle():
@@ -143,38 +103,38 @@ def test_gather3d_at_r3d18_size(engine, dtype, wname):
     To, Ho, Wo = _out_size(D, H, H, win)
     g = torch.Generator(device=dev)
     g.manual_seed(11)
-    ncdhw = torch.randn((nb * B, c, D, H, H), generator=g, device=dev).to(_T[dtype])
+    ncdhw = torch.randn((nb * B, c, D, H, H), generator=g, device=dev).to(GC.FMAP_DTYPES[dtype])
     r = np.random.RandomState(3)
     rt, rx, ry = (torch.as_tensor(r.randint(0, hi, (nb, P)).astype(np.int32), device=dev) for hi in (To, Ho, Wo))
     want = _torch_gather(ncdhw, rt, rx, ry, B, win, True)
     for path in ("ncdhw", "ndhwc_tma", "ndhwc_host", "ncdhw_host"):
         got = _gather(engine, path, ncdhw, rt, rx, ry, B, P, win, True)
         torch.cuda.synchronize()
-        _assert_same_bits(got, want)
+        GC.assert_same_bits(got, want)
         del got
     K = want.shape[1]
     wide = torch.full((want.shape[0], K + 40), 7.0, device=dev)
     _gather(engine, "ndhwc_tma", ncdhw, rt, rx, ry, B, P, win, True, out=wide[:, 8:8 + K])
     torch.cuda.synchronize()
-    _assert_same_bits(wide[:, 8:8 + K].contiguous(), want)
+    GC.assert_same_bits(wide[:, 8:8 + K].contiguous(), want)
     assert bool((wide[:, :8] == 7.0).all()) and bool((wide[:, 8 + K:] == 7.0).all())
 
 
-@pytest.mark.parametrize("dtype", list(_T))
+@pytest.mark.parametrize("dtype", list(GC.FMAP_DTYPES))
 @pytest.mark.parametrize("layout,host", [("ncdhw", False), ("ndhwc", False), ("ncdhw", True), ("ndhwc", True)])
 def test_point_gather3d_bits(engine, dtype, layout, host):
     dev = engine.device
     n, To, Ho, Wo, B, nb = 40, 4, 7, 6, 3, 2
-    y = _map((nb * B, n, To, Ho, Wo), dtype, 17 + n, dev)
-    rt, rx, ry, P = _points(nb, To, Ho, Wo, dev)
+    y = GC.special_map((nb * B, n, To, Ho, Wo), dtype, 17 + n, dev)
+    rt, rx, ry, P = GC.points3d(nb, To, Ho, Wo, dev)
     m = y if layout == "ncdhw" else y.permute(0, 2, 3, 4, 1).contiguous()
-    m = _pinned(m) if host else m
+    m = GC.pinned(m) if host else m
     got = engine.point_gather3d(m, rt, rx, ry, B, P, layout=layout)
     torch.cuda.synchronize()
     yc = y.float().cpu()
     want = torch.stack([yc[b * B + i, :, int(rt[b, p]), int(rx[b, p]), int(ry[b, p])]
                         for b in range(nb) for p in range(P) for i in range(B)])
-    _assert_same_bits(got, want)
+    GC.assert_same_bits(got, want)
 
 
 @pytest.mark.parametrize("wname", list(WINDOWS))
@@ -190,7 +150,7 @@ def test_gathered_x_reproduces_conv3d(engine, wname, layout):
     W2 = torch.randn((n, c) + _tr(k), generator=g, device=dev)
     b2 = torch.randn((n,), generator=g, device=dev)
     To, Ho, Wo = _out_size(D, H, W, win)
-    rt, rx, ry, P = _points(nb, To, Ho, Wo, dev)
+    rt, rx, ry, P = GC.points3d(nb, To, Ho, Wo, dev)
     m = x if layout == "ncdhw" else x.permute(0, 2, 3, 4, 1).contiguous()
     X = engine.patch_gather3d(m, rt, rx, ry, B, P, k, pad, stride, relu=True, layout=layout, dilation=dil)
     got = X.double() @ W2.reshape(n, -1).T.double() + b2.double()
@@ -249,10 +209,10 @@ def test_window_beyond_the_host_reader_is_refused(engine):
     dev = engine.device
     m = torch.randn(2, 8, 9, 9, 3, device=dev)
     geom = (8, 7, 7, 3, 3, 3, 1, 1, 1, 1, 1, 1)
-    rc, err = _raw_gather3d(engine, _pinned(m), 3, 8, 9, 9, 1, geom)
+    rc, err = _raw_gather3d(engine, GC.pinned(m), 3, 8, 9, 9, 1, geom)
     assert rc == engine.lib.CP_ERR_INVALID and "8x7x7" in err and "host reader" in err, err
     nc = m.permute(0, 4, 1, 2, 3).contiguous()
-    for mm, lay in ((m, 1), (nc, 0), (_pinned(nc), 0)):
+    for mm, lay in ((m, 1), (nc, 0), (GC.pinned(nc), 0)):
         rc, err = _raw_gather3d(engine, mm, 3, 8, 9, 9, lay, geom)
         assert rc == 0, err
     torch.cuda.synchronize()
@@ -292,11 +252,11 @@ def _profile_kernel_cases():
     for kind, (layout, host, c, names) in _KERNEL_CASES.items():
         for wname in names:
             k, pad, stride, dil = win = WINDOWS[wname]
-            rt, rx, ry, P = _points(nb, *_out_size(D, H, H, win), dev)
+            rt, rx, ry, P = GC.points3d(nb, *_out_size(D, H, H, win), dev)
             shape = (nb * B, D, H, H, c) if layout == "ndhwc" else (nb * B, c, D, H, H)
             m = torch.randn(shape, device=dev)
             if host:
-                m = _pinned(m)
+                m = GC.pinned(m)
             call = (lambda m=m, rt=rt, rx=rx, ry=ry, P=P, k=k, pad=pad, stride=stride, dil=dil, layout=layout:
                     engine.patch_gather3d(m, rt, rx, ry, B, P, k, pad, stride, layout=layout, dilation=dil))
             call()  # warm-up (module load)
@@ -315,21 +275,6 @@ def test_intended_kernels_run(engine):
     NDHWC pinned maps the host reader, NCDHW maps (HBM and pinned) the NCDHW kernel.  Each case runs _REPEAT times, so
     a lost activity record does not decide the check.  The session runs in a child process, so the suite's other
     profiler checks keep their record counts."""
-    import json
-    import os
-    import subprocess
-    import sys
-
-    here = os.path.dirname(os.path.abspath(__file__))
-    root = os.path.dirname(here)
-    code = ("import sys, json; sys.path[:0] = %r; import test_gpu_conv3d as t; "
-            "print('NAMES ' + json.dumps(t._profile_kernel_cases()))" % [root, os.path.join(root, "oracle"), here])
-    flags = ["-s"] if sys.flags.no_user_site else []
-    out = subprocess.run([sys.executable] + flags + ["-c", code], cwd=root, capture_output=True, text=True,
-                         timeout=600)
-    assert out.returncode == 0, out.stderr[-3000:]
-    names = json.loads([ln for ln in out.stdout.splitlines() if ln.startswith("NAMES ")][-1][6:])
-    names = [n.replace(" ", "") for n in names]
 
     def kind_of(n):
         for key, kind in (("patch_gather_ndhwc_tma<", "tma"), ("patch_gather_ndhwc_host<", "host"),
@@ -338,17 +283,9 @@ def test_intended_kernels_run(engine):
                 return kind
         return n
 
-    seen = [kind_of(n) for n in names]
-    assert set(seen) <= {"tma", "host", "simt", "ncdhw"}, sorted(set(names))
     want = {k: _REPEAT * len(v[3]) for k, v in _KERNEL_CASES.items()}
     want["ncdhw"] += want.pop("ncdhw_host")  # one kernel, two grids
-    LOST = 2
-    for kind, n in want.items():
-        assert n - LOST <= seen.count(kind) <= n, (kind, seen.count(kind), n, sorted(set(names)))
-
-
-def _rel(a, b):
-    return np.linalg.norm(a - b) / np.linalg.norm(b)
+    GC.assert_launch_counts(GC.launched_gather_kernels("test_gpu_conv3d"), kind_of, want)
 
 
 def _layer(name, c, n, D, H, k=3, pad=1, stride=1, dilation=1, N=1000, B=10, P=10, rank=None):
@@ -385,7 +322,7 @@ def test_dictionary_on_conv3d_layers_matches_oracle(engine, mode, tol, geom):
     assert cfgs.alpha == st.alpha
     assert after_oracle[2] == after_device[2] and np.array_equal(after_oracle[1], after_device[1])
     assert W.shape == oW.shape == (s.n, int(idxs.sum()), s.kt, s.kh, s.kw)
-    assert _rel(W, oW) <= tol and np.abs(B - oB).max() <= tol * max(1.0, np.abs(oB).max())
+    assert GC.rel(W, oW) <= tol and np.abs(B - oB).max() <= tol * max(1.0, np.abs(oB).max())
 
 
 def _video_layers(N=400, B=4, P=5):
@@ -401,42 +338,14 @@ def _video_layers(N=400, B=4, P=5):
             cpb200.synth.LayerShape("conv2d", 32, 24, 14, N=N, B=B, P=P)]
 
 
-class _Seeds:  # the oracle draws its CD seeds from an RNG object: feed it the pipeline's seed list
-    def __init__(self, seeds):
-        self.seeds, self.i = list(seeds), 0
-
-    def randint(self, lo, hi):
-        v = self.seeds[self.i]
-        self.i += 1
-        return v
-
-
 def _oracle_layer(s, d):
     """The oracle on one Conv3d pipeline problem: conv3d_oracle.gather3d (ReLU'd), then the oracle's dictionary with the
     problem's samples and seeds."""
-    import cp_oracle
-
     fm = d["fmap"].float().cpu().numpy() if d["layout"] == "ncdhw" else \
         d["fmap"].permute(0, 4, 1, 2, 3).float().cpu().numpy()
     pts = [d[k].cpu().numpy() for k in ("randt", "randx", "randy")]
     X = C3.gather3d(fm.astype(np.float64), *pts, s.B, s.k, s.pad, s.stride, s.dilation, relu=True)
-    newX = X.reshape((s.N, s.c) + s.window)
-    b2 = d["b2"].cpu().numpy()
-    st = O.DictState(alpha=1e-3)
-    info = {}
-    orig = cp_oracle.LassoCD.__init__
-
-    def patched(self, alpha, **kw):
-        orig(self, alpha, **kw)
-        self.rng = _Seeds(d["seeds"])
-
-    cp_oracle.LassoCD.__init__ = patched
-    try:
-        oi, oW, oB = C3.dictionary(newX, d["W2"].cpu().numpy(), d["feats"].cpu().numpy().astype(np.float64) - b2,
-                                   rank=s.rank, B2=b2, state=st, samples=d["samples"].cpu().numpy(), info=info)
-    finally:
-        cp_oracle.LassoCD.__init__ = orig
-    return oi, oW, oB, st.alpha, len(info["probes"])
+    return GC.oracle_on_problem(C3.dictionary, X.reshape((s.N, s.c) + s.window), s, d)
 
 
 @pytest.mark.parametrize("dtype", ["fp32", "bf16"])
@@ -455,7 +364,7 @@ def test_pipeline_on_conv3d_layers(engine, dtype, host_layout):
     for i, s in enumerate(shapes):
         hl = host_layout if isinstance(s, cpb200.synth.LayerShape3d) else "nchw"
         datas.append(cpb200.synth.make_problem_device(s, 70 + i, eng, pinned_host=True, host_layout=hl,
-                                                      dtype=_T[dtype]))
+                                                      dtype=GC.FMAP_DTYPES[dtype]))
     ref = pruner.prune_layers(eng, shapes, datas)
     torch.cuda.synchronize()
     ref = [(r.idxs.copy(), r.alpha, r.nprobe, r.W.cpu(), r.b.cpu()) for r in ref]
@@ -472,7 +381,7 @@ def test_pipeline_on_conv3d_layers(engine, dtype, host_layout):
             idxs, alpha, nprobe, W, b = ref[i]
             assert np.array_equal(idxs, oi) and alpha == oalpha and nprobe == onprobe, s.name
             W = W.numpy().reshape(oW.shape)
-            assert _rel(W, oW) <= 1e-7 and np.abs(b.numpy() - oB).max() <= 1e-7, s.name
+            assert GC.rel(W, oW) <= 1e-7 and np.abs(b.numpy() - oB).max() <= 1e-7, s.name
     eng.close()
 
 
@@ -490,7 +399,7 @@ def test_pipeline_with_tensor_core_statistics_matches_oracle(engine):
     torch.cuda.synchronize()
     oi, oW, oB, oalpha, onprobe = _oracle_layer(s, d)
     assert np.array_equal(r.idxs, oi) and r.alpha == oalpha and r.nprobe == onprobe
-    assert _rel(r.W.cpu().numpy().reshape(oW.shape), oW) <= 1e-4
+    assert GC.rel(r.W.cpu().numpy().reshape(oW.shape), oW) <= 1e-4
     assert np.abs(r.b.cpu().numpy() - oB).max() <= 1e-4 * max(1.0, np.abs(oB).max())
     eng.close()
 

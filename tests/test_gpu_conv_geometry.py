@@ -10,12 +10,12 @@ import pytest
 
 import conv_oracle as CO
 import cp_oracle as O
+import gather_checks as GC
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
 F = pytest.importorskip("torch.nn.functional")
 
-_T = {"fp32": torch.float32, "bf16": torch.bfloat16, "fp16": torch.float16}
 # (kernel_size, padding, stride, dilation), ints or (h, w) pairs as nn.Conv2d takes them
 WINDOWS = {
     "1x3": ((1, 3), (0, 1), 1, 1), "3x1": ((3, 1), (1, 0), 1, 1), "1x7": ((1, 7), (0, 3), 1, 1),
@@ -35,35 +35,6 @@ def _pair(v):
 def _out_size(H, W, win):
     (kh, kw), (ph, pw), (sh, sw), (dh, dw) = (_pair(v) for v in win)
     return (H + 2 * ph - dh * (kh - 1) - 1) // sh + 1, (W + 2 * pw - dw * (kw - 1) - 1) // sw + 1
-
-
-def _map(shape, dtype, seed, device):
-    """N(0,1) drawn in fp32 and rounded to dtype, with -0, +-inf, NaN and subnormals (of fp32, bf16 and fp16) seeded
-    in (the values of the existing gather tests)."""
-    g = torch.Generator(device=device)
-    g.manual_seed(seed)
-    fm = torch.randn(shape, generator=g, device=device)
-    flat = fm.view(-1)
-    specials = torch.tensor([-0.0, float("inf"), float("-inf"), float("nan"), 6e-8, -3e-6, 4e-5, 1e-39, -5e-39,
-                             1e-44], device=device)
-    idx = torch.randperm(flat.numel(), generator=g, device=device)[:max(len(specials), flat.numel() // 40)]
-    flat[idx] = specials[torch.arange(idx.numel(), device=device) % len(specials)]
-    return fm.to(_T[dtype])
-
-
-def _pinned(t):
-    h = torch.empty(t.shape, dtype=t.dtype, pin_memory=True)
-    h.copy_(t)
-    return h
-
-
-def _assert_same_bits(got, want):
-    """Bit equality (so -0 and +0 differ); NaN positions compared separately, their payloads not."""
-    assert got.dtype == want.dtype == torch.float32 and got.shape == want.shape
-    ng, nw = torch.isnan(got), torch.isnan(want)
-    assert torch.equal(ng, nw)
-    z = torch.zeros_like(got)
-    assert torch.equal(torch.where(ng, z, got).view(torch.int32), torch.where(nw, z, want).view(torch.int32))
 
 
 def _points(nb, Ho, Wo, device):
@@ -117,12 +88,12 @@ def _gather(engine, path, nchw, rx, ry, B, P, win, relu, out=None):
     layout, host, _ = PATHS[path]
     m = nchw if layout == "nchw" else nchw.permute(0, 2, 3, 1).contiguous()
     if host:
-        m = _pinned(m)
+        m = GC.pinned(m)
     k, pad, stride, dil = win
     return engine.patch_gather(m, rx, ry, B, P, k, pad, stride, relu=relu, layout=layout, dilation=dil, out=out)
 
 
-@pytest.mark.parametrize("dtype", list(_T))
+@pytest.mark.parametrize("dtype", list(GC.FMAP_DTYPES))
 @pytest.mark.parametrize("path", list(PATHS))
 @pytest.mark.parametrize("wname", list(WINDOWS))
 def test_conv_gather_bits_equal_unfold(engine, dtype, path, wname):
@@ -131,12 +102,13 @@ def test_conv_gather_bits_equal_unfold(engine, dtype, path, wname):
     c = PATHS[path][2]
     H, W, B, nb = 11, 10, 3, 2
     Ho, Wo = _out_size(H, W, win)
-    nchw = _map((nb * B, c, H, W), dtype, zlib.crc32(("%s/%s/%s" % (wname, path, dtype)).encode()) % 10007, dev)
+    seed = zlib.crc32(("%s/%s/%s" % (wname, path, dtype)).encode()) % 10007
+    nchw = GC.special_map((nb * B, c, H, W), dtype, seed, dev)
     rx, ry, P = _points(nb, Ho, Wo, dev)
     for relu in (False, True):
         got = _gather(engine, path, nchw, rx, ry, B, P, win, relu)
         torch.cuda.synchronize()
-        _assert_same_bits(got.cpu(), _unfold_oracle(nchw, rx, ry, B, win, relu))
+        GC.assert_same_bits(got.cpu(), _unfold_oracle(nchw, rx, ry, B, win, relu))
 
 
 @pytest.mark.parametrize("dtype", ["fp32", "bf16"])
@@ -150,27 +122,27 @@ def test_conv_gather_at_deeplab_size(engine, dtype, wname):
     Ho, Wo = _out_size(H, H, win)
     g = torch.Generator(device=dev)
     g.manual_seed(11)
-    nchw = torch.randn((nb * B, c, H, H), generator=g, device=dev).to(_T[dtype])
+    nchw = torch.randn((nb * B, c, H, H), generator=g, device=dev).to(GC.FMAP_DTYPES[dtype])
     r = np.random.RandomState(3)
     rx = torch.as_tensor(r.randint(0, Ho, (nb, P)).astype(np.int32), device=dev)
     ry = torch.as_tensor(r.randint(0, Wo, (nb, P)).astype(np.int32), device=dev)
     want = _direct_oracle(nchw, rx, ry, B, win)
     small = slice(0, 2 * P * B)
-    _assert_same_bits(want[small], _unfold_oracle(nchw[:2 * B], rx[:2], ry[:2], B, win, True))
+    GC.assert_same_bits(want[small], _unfold_oracle(nchw[:2 * B], rx[:2], ry[:2], B, win, True))
     for path in ("nchw", "nhwc_tma", "nhwc_host"):
         got = _gather(engine, path, nchw, rx, ry, B, P, win, True)
         torch.cuda.synchronize()
-        _assert_same_bits(got.cpu(), want)
+        GC.assert_same_bits(got.cpu(), want)
         del got
     K = want.shape[1]
     wide = torch.full((want.shape[0], K + 40), 7.0, device=dev)
     _gather(engine, "nhwc_tma", nchw, rx, ry, B, P, win, True, out=wide[:, 8:8 + K])
     torch.cuda.synchronize()
-    _assert_same_bits(wide[:, 8:8 + K].contiguous().cpu(), want)
+    GC.assert_same_bits(wide[:, 8:8 + K].contiguous().cpu(), want)
     assert bool((wide[:, :8] == 7.0).all()) and bool((wide[:, 8 + K:] == 7.0).all())
 
 
-@pytest.mark.parametrize("dtype", list(_T))
+@pytest.mark.parametrize("dtype", list(GC.FMAP_DTYPES))
 @pytest.mark.parametrize("path", list(PATHS))
 @pytest.mark.parametrize("k,pad,stride", [(1, 0, 1), (1, 0, 2), (3, 1, 1), (3, 0, 2), (5, 2, 1)])
 def test_square_windows_give_the_reference_entries_bits(engine, dtype, path, k, pad, stride):
@@ -181,16 +153,16 @@ def test_square_windows_give_the_reference_entries_bits(engine, dtype, path, k, 
     layout, host, _ = PATHS[path]
     H, B, nb = 9, 3, 2
     Ho = (H + 2 * pad - k) // stride + 1
-    nchw = _map((nb * B, c, H, H), dtype, c + k * 7 + stride, dev)
+    nchw = GC.special_map((nb * B, c, H, H), dtype, c + k * 7 + stride, dev)
     rx, ry, P = _points(nb, Ho, Ho, dev)
     for relu in (False, True):
         a = _gather(engine, path, nchw, rx, ry, B, P, (k, pad, stride, 1), relu)
         b = _gather(engine, path, nchw, rx, ry, B, P, ((k, k), (pad, pad), (stride, stride), (1, 1)), relu)
         torch.cuda.synchronize()
-        _assert_same_bits(b, a)
+        GC.assert_same_bits(b, a)
         if dtype == "fp32":
             m = nchw if layout == "nchw" else nchw.permute(0, 2, 3, 1).contiguous()
-            m = _pinned(m) if host else m
+            m = GC.pinned(m) if host else m
             X = torch.empty_like(a)
             ffi, lib = engine.ffi, engine.lib
             rc = lib.cp_patch_gather(engine.h, ffi.cast("const float*", m.data_ptr()), nb, B, c, H, H,
@@ -199,7 +171,7 @@ def test_square_windows_give_the_reference_entries_bits(engine, dtype, path, k, 
                                      ffi.cast("float*", X.data_ptr()), X.stride(0), ffi.NULL)
             assert rc == 0
             torch.cuda.synchronize()
-            _assert_same_bits(X, a)
+            GC.assert_same_bits(X, a)
 
 
 def _raw_gather(engine, m, c, H, W, layout, kh, kw, ph, pw, sh, sw, dh, dw, entry="conv"):
@@ -239,11 +211,11 @@ def test_window_beyond_the_host_reader_is_refused(engine):
 
     dev = engine.device
     m = torch.randn(2, 12, 12, 3, device=dev)
-    rc, err = _raw_gather(engine, _pinned(m), 3, 12, 12, 1, 9, 10, 4, 4, 1, 1, 1, 1)
+    rc, err = _raw_gather(engine, GC.pinned(m), 3, 12, 12, 1, 9, 10, 4, 4, 1, 1, 1, 1)
     assert rc == engine.lib.CP_ERR_INVALID and "kernel_size 9x10" in err and "host reader" in err, err
     r = torch.zeros((1, 1), dtype=torch.int32, device=dev)
     with pytest.raises(cpb200._cabi.CpError):
-        engine.patch_gather(_pinned(m), r, r, 2, 1, (9, 10), 4, 1, layout="nhwc")
+        engine.patch_gather(GC.pinned(m), r, r, 2, 1, (9, 10), 4, 1, layout="nhwc")
     for mm, lay in ((m, 1), (m.permute(0, 3, 1, 2).contiguous(), 0)):
         rc, err = _raw_gather(engine, mm, 3, 12, 12, lay, 9, 10, 4, 4, 1, 1, 1, 1)
         assert rc == 0, err
@@ -252,18 +224,18 @@ def test_window_beyond_the_host_reader_is_refused(engine):
     torch.cuda.synchronize()
 
 
-@pytest.mark.parametrize("dtype", list(_T))
+@pytest.mark.parametrize("dtype", list(GC.FMAP_DTYPES))
 def test_largest_nhwc_simt_window_equals_unfold(engine, dtype):
     """kh*kw = 95, the largest window the 2-D entries take on the NHWC SIMT kernel in HBM (kw = 19 is beyond TMA), over
     c = 140 channels (a full and a partial channel tile), against F.unfold."""
     win = ((5, 19), (2, 9), 1, 1)
     H, W, B, nb = 9, 21, 3, 2
-    nchw = _map((nb * B, 140, H, W), dtype, 95, engine.device)
+    nchw = GC.special_map((nb * B, 140, H, W), dtype, 95, engine.device)
     rx, ry, P = _points(nb, *_out_size(H, W, win), engine.device)
     for relu in (False, True):
         got = _gather(engine, "nhwc_simt", nchw, rx, ry, B, P, win, relu)
         torch.cuda.synchronize()
-        _assert_same_bits(got.cpu(), _unfold_oracle(nchw, rx, ry, B, win, relu))
+        GC.assert_same_bits(got.cpu(), _unfold_oracle(nchw, rx, ry, B, win, relu))
 
 
 def test_reference_entries_still_refuse_even_kernels(engine):
@@ -304,7 +276,7 @@ def _profile_kernel_cases():
             rx, ry, P = _points(nb, Ho, Wo, dev)
             m = torch.randn((nb * B, H, H, c), device=dev)
             if kind == "host":
-                m = _pinned(m)
+                m = GC.pinned(m)
             call = (lambda m=m, rx=rx, ry=ry, P=P, k=k, pad=pad, stride=stride, dil=dil:
                     engine.patch_gather(m, rx, ry, B, P, k, pad, stride, layout="nhwc", dilation=dil))
             call()  # warm-up (module load)
@@ -323,21 +295,6 @@ def test_intended_kernels_run(engine):
     the NHWC SIMT kernel, NHWC pinned maps the host reader.  Each case runs _REPEAT times, so a lost activity record
     does not decide the check.  The session runs in a child process: a process that has profiled once loses more
     activity records in its later sessions, and other tests of the suite profile too."""
-    import json
-    import os
-    import subprocess
-    import sys
-
-    here = os.path.dirname(os.path.abspath(__file__))
-    root = os.path.dirname(here)
-    code = ("import sys, json; sys.path[:0] = %r; import test_gpu_conv_geometry as t; "
-            "print('NAMES ' + json.dumps(t._profile_kernel_cases()))" % [root, os.path.join(root, "oracle"), here])
-    flags = ["-s"] if sys.flags.no_user_site else []
-    out = subprocess.run([sys.executable] + flags + ["-c", code], cwd=root, capture_output=True, text=True,
-                         timeout=600)
-    assert out.returncode == 0, out.stderr[-3000:]
-    names = json.loads([ln for ln in out.stdout.splitlines() if ln.startswith("NAMES ")][-1][6:])
-    names = [n.replace(" ", "") for n in names]
 
     def kind_of(n):
         if "patch_gather_nhwc_tma<" in n:
@@ -348,12 +305,8 @@ def test_intended_kernels_run(engine):
             return "simt"
         return n
 
-    seen = [kind_of(n) for n in names]
-    assert set(seen) <= set(_KERNEL_CASES), sorted(set(names))
-    LOST = 2
-    for kind, cases in _KERNEL_CASES.items():
-        want = _REPEAT * len(cases)
-        assert want - LOST <= seen.count(kind) <= want, (kind, seen.count(kind), want, sorted(set(names)))
+    want = {kind: _REPEAT * len(cases) for kind, cases in _KERNEL_CASES.items()}
+    GC.assert_launch_counts(GC.launched_gather_kernels("test_gpu_conv_geometry"), kind_of, want)
 
 
 @pytest.mark.parametrize("wname", list(WINDOWS))
@@ -377,10 +330,6 @@ def test_gathered_x_reproduces_the_convolution(engine, wname):
     want = torch.stack([y[b * B + i, :, int(rx[b, p]), int(ry[b, p])] for b in range(nb) for p in range(P)
                         for i in range(B)])
     torch.testing.assert_close(got, want, rtol=1e-5, atol=1e-5)
-
-
-def _rel(a, b):
-    return np.linalg.norm(a - b) / np.linalg.norm(b)
 
 
 def _layer(name, c, n, H, k, pad, stride=1, dilation=1, N=1000, B=10, P=10, rank=None):
@@ -417,7 +366,7 @@ def test_dictionary_on_dilated_and_rectangular_layers_matches_oracle(engine, mod
     assert cfgs.alpha == st.alpha
     assert after_oracle[2] == after_device[2] and np.array_equal(after_oracle[1], after_device[1])
     assert W.shape == oW.shape == (s.n, int(idxs.sum()), s.kh, s.kw)
-    assert _rel(W, oW) <= tol and np.abs(B - oB).max() <= tol * max(1.0, np.abs(oB).max())
+    assert GC.rel(W, oW) <= tol and np.abs(B - oB).max() <= tol * max(1.0, np.abs(oB).max())
 
 
 def _deeplab_inception_layers(N=600, B=4, P=5):
@@ -433,22 +382,10 @@ def _deeplab_inception_layers(N=600, B=4, P=5):
             _layer("s21", 32, 16, 14, 3, 1, stride=(2, 1), N=400, B=B, P=P)]
 
 
-class _Seeds:  # the oracle draws its CD seeds from an RNG object: feed it the pipeline's seed list
-    def __init__(self, seeds):
-        self.seeds, self.i = list(seeds), 0
-
-    def randint(self, lo, hi):
-        v = self.seeds[self.i]
-        self.i += 1
-        return v
-
-
 def _oracle_layer(s, d):
     """The oracle on one pipeline problem: extract_XY_conv with the layer's window, ReLU, oracle.dictionary with the
     problem's samples and seeds (what oracle.dictionary_kernel does for square layers)."""
     import types
-
-    import cp_oracle
 
     fm = d["fmap"].float().cpu().numpy() if d.get("layout", "nchw") == "nchw" else \
         d["fmap"].permute(0, 3, 1, 2).float().cpu().numpy()
@@ -459,22 +396,7 @@ def _oracle_layer(s, d):
     spec = types.SimpleNamespace(name="y", kernel_size=s.k, pad=s.pad, stride=s.stride, dilation=s.dilation)
     X = CO.extract_XY_conv(lambda b: {"x": fm[b * s.B:(b + 1) * s.B]}, "x", spec, pd)
     newX = O.relu(np.rollaxis(X.reshape((-1, s.kh, s.kw, X.shape[1])), 3, 1).copy())
-    b2 = d["b2"].cpu().numpy()
-    st = O.DictState(alpha=1e-3)
-    info = {}
-    orig = cp_oracle.LassoCD.__init__
-
-    def patched(self, alpha, **kw):
-        orig(self, alpha, **kw)
-        self.rng = _Seeds(d["seeds"])
-
-    cp_oracle.LassoCD.__init__ = patched
-    try:
-        oi, oW, oB = CO.dictionary(newX, d["W2"].cpu().numpy(), d["feats"].cpu().numpy().astype(np.float64) - b2,
-                                  rank=s.rank, B2=b2, state=st, samples=d["samples"].cpu().numpy(), info=info)
-    finally:
-        cp_oracle.LassoCD.__init__ = orig
-    return oi, oW, oB, st.alpha, len(info["probes"])
+    return GC.oracle_on_problem(CO.dictionary, newX, s, d)
 
 
 @pytest.mark.parametrize("host_layout", ["nchw", "nhwc"])
@@ -506,7 +428,7 @@ def test_pipeline_on_deeplab_and_inception_layers(engine, host_layout):
             idxs, alpha, nprobe, W, b = ref[i]
             assert np.array_equal(idxs, oi) and alpha == oalpha and nprobe == onprobe, s.name
             W = W.numpy().reshape(oW.shape)
-            assert _rel(W, oW) <= 1e-7 and np.abs(b.numpy() - oB).max() <= 1e-7, s.name
+            assert GC.rel(W, oW) <= 1e-7 and np.abs(b.numpy() - oB).max() <= 1e-7, s.name
     eng.close()
 
 
@@ -554,4 +476,4 @@ def test_net_with_dilated_and_rectangular_convs_matches_oracle(engine):
                                   B2=biases[Y_name], state=st)
         assert np.array_equal(idxs, oi) and cfgs.alpha == st.alpha, Y_name
         assert W.shape == oW.shape == (co, int(oi.sum()), kh, kw)
-        assert _rel(W, oW) <= 1e-7 and np.abs(B - oB).max() <= 1e-7, Y_name
+        assert GC.rel(W, oW) <= 1e-7 and np.abs(B - oB).max() <= 1e-7, Y_name

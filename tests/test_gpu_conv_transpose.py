@@ -10,13 +10,12 @@ import pytest
 
 import conv3d_oracle as C3
 import cp_oracle as O
-import test_gpu_conv3d as G3
+import gather_checks as GC
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
 F = pytest.importorskip("torch.nn.functional")
 
-_T = G3._T
 # (kernel_size, padding, stride, dilation, output_padding) as nn.ConvTranspose2d / 3d take them
 GEOMS2D = {
     "k2s2": (2, 0, 2, 1, 0), "k4s2p1": (4, 1, 2, 1, 0), "k3s2p1op1": (3, 1, 2, 1, 1), "k3s2d2": (3, 0, 2, 2, 0),
@@ -69,7 +68,7 @@ def _gather(engine, path, ncdhw, pts, B, P, geom, relu, d3, out=None):
     clast, host, _ = PATHS[path]
     m = ncdhw.permute(0, *range(2, ncdhw.dim()), 1).contiguous() if clast else ncdhw
     if host:
-        m = G3._pinned(m)
+        m = GC.pinned(m)
     k, pad, stride, dil, _ = geom
     if d3:
         return engine.patch_gather3d(m, *pts, B, P, k, pad, stride, relu=relu, layout="ndhwc" if clast else "ncdhw",
@@ -78,7 +77,7 @@ def _gather(engine, path, ncdhw, pts, B, P, geom, relu, d3, out=None):
                                dilation=dil, out=out, transposed=True)
 
 
-@pytest.mark.parametrize("dtype", list(_T))
+@pytest.mark.parametrize("dtype", list(GC.FMAP_DTYPES))
 @pytest.mark.parametrize("path", list(PATHS))
 @pytest.mark.parametrize("gname", ["2d:" + n for n in GEOMS2D] + ["3d:" + n for n in GEOMS3D])
 def test_gather_tr_bits_equal_reference(engine, dtype, path, gname):
@@ -91,19 +90,19 @@ def test_gather_tr_bits_equal_reference(engine, dtype, path, gname):
     if d3:
         D, H, W = 3, 5, 4
         To, Ho, Wo = _out_size((D, H, W), geom)
-        x = G3._map((nb * B, c, D, H, W), dtype, seed, dev)
-        rt, rx, ry, P = G3._points(nb, To, Ho, Wo, dev)
+        x = GC.special_map((nb * B, c, D, H, W), dtype, seed, dev)
+        rt, rx, ry, P = GC.points3d(nb, To, Ho, Wo, dev)
         pts = (rt, rx, ry)
     else:
         H, W = 6, 5
         Ho, Wo = _out_size((H, W), geom)
-        x = G3._map((nb * B, c, H, W), dtype, seed, dev)
+        x = GC.special_map((nb * B, c, H, W), dtype, seed, dev)
         rx, ry, P = _points2d(nb, Ho, Wo, dev)
         pts = (rx, ry)
     for relu in (False, True):
         got = _gather(engine, path, x, pts, B, P, geom, relu, d3)
         torch.cuda.synchronize()
-        G3._assert_same_bits(got, _ref(x, pts, B, geom, relu, d3))
+        GC.assert_same_bits(got, _ref(x, pts, B, geom, relu, d3))
 
 
 @pytest.mark.parametrize("dtype", ["fp32", "bf16"])
@@ -119,21 +118,21 @@ def test_gather_tr_at_decoder_size(engine, dtype, gname):
     out = _out_size(dims, geom)
     g = torch.Generator(device=dev)
     g.manual_seed(11)
-    x = torch.randn((nb * B, c) + dims, generator=g, device=dev).to(_T[dtype])
+    x = torch.randn((nb * B, c) + dims, generator=g, device=dev).to(GC.FMAP_DTYPES[dtype])
     r = np.random.RandomState(3)
     pts = tuple(torch.as_tensor(r.randint(0, hi, (nb, P)).astype(np.int32), device=dev) for hi in out)
     want = _ref(x, pts, B, geom, True, d3)
     for path in ("cf", "cf_host", "cl", "cl_host"):
         got = _gather(engine, path, x, pts, B, P, geom, True, d3)
         torch.cuda.synchronize()
-        G3._assert_same_bits(got, want)
+        GC.assert_same_bits(got, want)
         del got
     K = want.shape[1]
     for path in ("cf", "cl"):
         wide = torch.full((want.shape[0], K + 40), 7.0, device=dev)
         _gather(engine, path, x, pts, B, P, geom, True, d3, out=wide[:, 8:8 + K])
         torch.cuda.synchronize()
-        G3._assert_same_bits(wide[:, 8:8 + K].contiguous(), want)
+        GC.assert_same_bits(wide[:, 8:8 + K].contiguous(), want)
         assert bool((wide[:, :8] == 7.0).all()) and bool((wide[:, 8 + K:] == 7.0).all())
 
 
@@ -145,12 +144,12 @@ def test_gather_tr_channel_tiles(engine, dtype, path):
     dev = engine.device
     geom = GEOMS2D["k3s1p1"]
     B, nb = 2, 1
-    x = G3._map((nb * B, 1400, 6, 5), dtype, 3, dev)
+    x = GC.special_map((nb * B, 1400, 6, 5), dtype, 3, dev)
     rx, ry, P = _points2d(nb, *_out_size((6, 5), geom), dev)
     for relu in (False, True):
         got = _gather(engine, path, x, (rx, ry), B, P, geom, relu, False)
         torch.cuda.synchronize()
-        G3._assert_same_bits(got, _ref(x, (rx, ry), B, geom, relu, False))
+        GC.assert_same_bits(got, _ref(x, (rx, ry), B, geom, relu, False))
 
 
 @pytest.mark.parametrize("gname", ["2d:" + n for n in GEOMS2D] + ["3d:" + n for n in GEOMS3D])
@@ -169,7 +168,7 @@ def test_gathered_x_reproduces_conv_transpose(engine, gname, clast):
     b2 = torch.randn((n,), generator=g, device=dev)
     out = _out_size(dims, geom)
     if d3:
-        rt, rx, ry, P = G3._points(nb, *out, dev)
+        rt, rx, ry, P = GC.points3d(nb, *out, dev)
         pts = (rt, rx, ry)
     else:
         rx, ry, P = _points2d(nb, *out, dev)
@@ -263,7 +262,7 @@ def test_window_wider_than_the_map_is_gathered(engine):
     for path in ("cf", "cl"):
         got = _gather(engine, path, x, (rx, ry), 2, P, geom, False, False)
         torch.cuda.synchronize()
-        G3._assert_same_bits(got, _ref(x, (rx, ry), 2, geom, False, False))
+        GC.assert_same_bits(got, _ref(x, (rx, ry), 2, geom, False, False))
 
 
 # kind -> (channels last, d3, channels, geometries); each runs from HBM and from pinned host memory
@@ -288,7 +287,7 @@ def _profile_kernel_cases():
             dims = (3, 6, 6) if d3 else (8, 8)
             out = _out_size(dims, geom)
             if d3:
-                rt, rx, ry, P = G3._points(nb, *out, dev)
+                rt, rx, ry, P = GC.points3d(nb, *out, dev)
                 pts = (rt, rx, ry)
             else:
                 rx, ry, P = _points2d(nb, *out, dev)
@@ -296,7 +295,7 @@ def _profile_kernel_cases():
             x = torch.randn((nb * B, c) + dims, device=dev)
             for host in (False, True):
                 m = x.permute(0, *range(2, x.dim()), 1).contiguous() if clast else x
-                m = G3._pinned(m) if host else m
+                m = GC.pinned(m) if host else m
                 lay = ("ndhwc" if d3 else "nhwc") if clast else ("ncdhw" if d3 else "nchw")
                 k, pad, stride, dil, _ = geom
                 fn = engine.patch_gather3d if d3 else engine.patch_gather
@@ -316,21 +315,6 @@ def _profile_kernel_cases():
 def test_intended_kernels_run(engine):
     """One profiler session (in a child process, so the suite's other profiler checks keep their record counts): each
     layout and rank launches its own kernel, from HBM and from pinned host memory alike."""
-    import json
-    import os
-    import subprocess
-    import sys
-
-    here = os.path.dirname(os.path.abspath(__file__))
-    root = os.path.dirname(here)
-    code = ("import sys, json; sys.path[:0] = %r; import test_gpu_conv_transpose as t; "
-            "print('NAMES ' + json.dumps(t._profile_kernel_cases()))" % [root, os.path.join(root, "oracle"), here])
-    flags = ["-s"] if sys.flags.no_user_site else []
-    out = subprocess.run([sys.executable] + flags + ["-c", code], cwd=root, capture_output=True, text=True,
-                         timeout=600)
-    assert out.returncode == 0, out.stderr[-3000:]
-    names = json.loads([ln for ln in out.stdout.splitlines() if ln.startswith("NAMES ")][-1][6:])
-    names = [n.replace(" ", "") for n in names]
 
     def kind_of(n):
         for kind in ("ncdhw", "nchw", "ndhwc", "nhwc"):
@@ -338,12 +322,8 @@ def test_intended_kernels_run(engine):
                 return kind
         return n
 
-    seen = [kind_of(n) for n in names]
-    assert set(seen) <= set(_KERNEL_CASES), sorted(set(names))
-    LOST = 2
-    for kind, v in _KERNEL_CASES.items():
-        n = 2 * _REPEAT * len(v[3])
-        assert n - LOST <= seen.count(kind) <= n, (kind, seen.count(kind), n, sorted(set(names)))
+    want = {kind: 2 * _REPEAT * len(v[3]) for kind, v in _KERNEL_CASES.items()}  # HBM and pinned host
+    GC.assert_launch_counts(GC.launched_gather_kernels("test_gpu_conv_transpose"), kind_of, want)
 
 
 # ----------------------------------------------------------------------------- solver and pipeline
@@ -385,14 +365,12 @@ def test_dictionary_on_transposed_layers_matches_oracle(engine, mode, tol, geo):
     assert cfgs.alpha == st.alpha
     assert after_oracle[2] == after_device[2] and np.array_equal(after_oracle[1], after_device[1])
     assert W.shape == oW.shape
-    assert G3._rel(W, oW) <= tol and np.abs(B - oB).max() <= tol * max(1.0, np.abs(oB).max())
+    assert GC.rel(W, oW) <= tol and np.abs(B - oB).max() <= tol * max(1.0, np.abs(oB).max())
 
 
 def _oracle_layer(s, d):
     """The oracle on one pipeline problem of a transposed layer: synth's numpy transposed gather (fp64, ReLU'd), then
     conv3d_oracle.dictionary with the problem's samples and seeds."""
-    import cp_oracle
-
     import cpb200
 
     d3 = hasattr(s, "kt")
@@ -406,22 +384,7 @@ def _oracle_layer(s, d):
     else:
         pts = [d[k].cpu().numpy() for k in ("randx", "randy")]
         X = cpb200.synth.gather_patches_tr_numpy(fm, *pts, s.B, s.k, s.pad, s.stride, True, dilation=s.dilation)
-    b2 = d["b2"].cpu().numpy()
-    st = O.DictState(alpha=1e-3)
-    info = {}
-    orig = cp_oracle.LassoCD.__init__
-
-    def patched(self, alpha, **kw):
-        orig(self, alpha, **kw)
-        self.rng = G3._Seeds(d["seeds"])
-
-    cp_oracle.LassoCD.__init__ = patched
-    try:
-        oi, oW, oB = C3.dictionary(X, d["W2"].cpu().numpy(), d["feats"].cpu().numpy().astype(np.float64) - b2,
-                                   rank=s.rank, B2=b2, state=st, samples=d["samples"].cpu().numpy(), info=info)
-    finally:
-        cp_oracle.LassoCD.__init__ = orig
-    return oi, oW, oB, st.alpha, len(info["probes"])
+    return GC.oracle_on_problem(C3.dictionary, X, s, d)
 
 
 def _decoder_layers(N=800, B=4, P=10):
@@ -449,7 +412,7 @@ def test_pipeline_on_transposed_layers(engine, dtype, host_layout):
     eng.gram_mode = 0
     shapes = _decoder_layers()
     datas = [cpb200.synth.make_problem_device(s, 90 + i, eng, pinned_host=True, host_layout=host_layout,
-                                              dtype=_T[dtype]) for i, s in enumerate(shapes)]
+                                              dtype=GC.FMAP_DTYPES[dtype]) for i, s in enumerate(shapes)]
     ref = pruner.prune_layers(eng, shapes, datas)
     torch.cuda.synchronize()
     assert [r.info["verdict"] for r in ref] == ["ok"] * len(shapes)
@@ -467,7 +430,7 @@ def test_pipeline_on_transposed_layers(engine, dtype, host_layout):
             oi, oW, oB, oalpha, onprobe = _oracle_layer(s, d)
             idxs, alpha, nprobe, W, b = ref[i]
             assert np.array_equal(idxs, oi) and alpha == oalpha and nprobe == onprobe, s.name
-            assert G3._rel(W.numpy().reshape(oW.shape), oW) <= 1e-7 and np.abs(b.numpy() - oB).max() <= 1e-7, s.name
+            assert GC.rel(W.numpy().reshape(oW.shape), oW) <= 1e-7 and np.abs(b.numpy() - oB).max() <= 1e-7, s.name
     eng.close()
 
 
@@ -522,7 +485,7 @@ def _run_one(s, d, mode):
 def _check_against_oracle(s, d, r, tol):
     oi, oW, oB, oalpha, onprobe = _oracle_layer(s, d)
     assert np.array_equal(r.idxs, oi) and r.alpha == oalpha and r.nprobe == onprobe
-    assert G3._rel(r.W.cpu().numpy().reshape(oW.shape), oW) <= tol
+    assert GC.rel(r.W.cpu().numpy().reshape(oW.shape), oW) <= tol
     assert np.abs(r.b.cpu().numpy() - oB).max() <= tol * max(1.0, np.abs(oB).max())
 
 

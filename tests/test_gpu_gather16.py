@@ -5,6 +5,7 @@ import numpy as np
 import pytest
 
 import cases
+import gather_checks as GC
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
@@ -27,15 +28,6 @@ def _map16(shape, dtype, seed, device):
     idx = torch.randperm(flat.numel(), generator=g, device=device)[:max(len(specials), flat.numel() // 40)]
     flat[idx] = specials[torch.arange(idx.numel(), device=device) % len(specials)]
     return fm.to(_T[dtype])
-
-
-def _assert_same_bits(got, want):
-    """Bit equality (so -0 and +0 differ); NaN positions compared separately, their payloads not."""
-    assert got.dtype == want.dtype == torch.float32 and got.shape == want.shape
-    ng, nw = torch.isnan(got), torch.isnan(want)
-    assert torch.equal(ng, nw)
-    z = torch.zeros_like(got)
-    assert torch.equal(torch.where(ng, z, got).view(torch.int32), torch.where(nw, z, want).view(torch.int32))
 
 
 def _points(nb, Ho, device):
@@ -63,43 +55,54 @@ def test_patch_gather_of_16bit_map_equals_gather_of_widened_map(engine, dtype, c
         for relu in (False, True):
             want = engine.patch_gather(a32, rx, ry, B, P, k, pad, stride, relu=relu, layout=layout)
             got = engine.patch_gather(a16, rx, ry, B, P, k, pad, stride, relu=relu, layout=layout)
-            _assert_same_bits(got, want)
+            GC.assert_same_bits(got, want)
             if relu:
                 assert not bool(torch.isnan(got).any())  # fmaxf(NaN, 0) = 0, as in the fp32 kernel
 
 
 PATH_SHAPES = [(16, 3), (24, 5), (64, 1), (512, 3), (2048, 1), (20, 3), (12, 3)]
+_PATH_CASES = [(dtype, c, k) for dtype in ("bf16", "fp16") for c, k in PATH_SHAPES]
+
+
+def _profile_kernel_cases():
+    """Gathers every case of _PATH_CASES once inside one profiler session, after a warm-up whose bits are checked
+    against the gather of the widened map; returns the gather kernels' names in launch order."""
+    import cpb200
+    from torch.profiler import ProfilerActivity, profile
+
+    engine = cpb200.get_engine()
+    dev = engine.device
+    H, B, nb, stride = 7, 2, 2, 1
+    rx, ry, P = _points(nb, H, dev)
+    runs = []
+    for dtype, c, k in _PATH_CASES:
+        m16 = _map16((nb * B, H, H, c), dtype, c + k, dev)
+        out = engine.patch_gather(m16, rx, ry, B, P, k, k // 2, stride, layout="nhwc")  # warm-up (module load)
+        want = engine.patch_gather(m16.float(), rx, ry, B, P, k, k // 2, stride, layout="nhwc")
+        GC.assert_same_bits(out, want)
+        runs.append((k, m16, out))
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for k, m16, out in runs:
+            engine.patch_gather(m16, rx, ry, B, P, k, k // 2, stride, layout="nhwc", out=out)
+        torch.cuda.synchronize()
+    kernels = sorted((e for e in prof.events() if "patch_gather" in e.name and e.device_type.name == "CUDA"),
+                     key=lambda e: e.time_range.start)
+    return [e.name for e in kernels]
 
 
 def test_16bit_nhwc_path_is_the_one_its_shape_selects(engine):
     """c % 8 == 0 and c >= 16: the TMA kernel must be what ran (a silent SIMT fall-back would pass the bit checks
     above).  c = 20 takes TMA as fp32 but not in 16 bit (40-byte channel stride); c = 12 never does.  One profiler
-    session for every case: the launches run in order on one stream, so the i-th kernel belongs to the i-th case."""
-    from torch.profiler import ProfilerActivity, profile
-
-    dev = engine.device
-    H, B, nb, stride = 7, 2, 2, 1
-    rx, ry, P = _points(nb, H, dev)
-    runs = []
-    for dtype in ("bf16", "fp16"):
-        for c, k in PATH_SHAPES:
-            m16 = _map16((nb * B, H, H, c), dtype, c + k, dev)
-            out = engine.patch_gather(m16, rx, ry, B, P, k, k // 2, stride, layout="nhwc")  # warm-up (module load)
-            want = engine.patch_gather(m16.float(), rx, ry, B, P, k, k // 2, stride, layout="nhwc")
-            _assert_same_bits(out, want)
-            runs.append((dtype, c, k, m16, out))
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for dtype, c, k, m16, out in runs:
-            engine.patch_gather(m16, rx, ry, B, P, k, k // 2, stride, layout="nhwc", out=out)
-        torch.cuda.synchronize()
-    kernels = sorted((e for e in prof.events() if "patch_gather" in e.name and e.device_type.name == "CUDA"),
-                     key=lambda e: e.time_range.start)
-    assert len(kernels) == len(runs), [e.name for e in kernels]
-    for (dtype, c, k, _, _), e in zip(runs, kernels):
+    session for every case: the launches run in order on one stream, so the i-th kernel belongs to the i-th case.  The
+    session runs in a child process: a process that has profiled once may lose activity records in its later
+    sessions, and this check counts every launch."""
+    names = GC.launched_gather_kernels("test_gpu_gather16")
+    assert len(names) == len(_PATH_CASES), names
+    for (dtype, c, k), n in zip(_PATH_CASES, names):
         tma = c % 8 == 0 and c >= 16
-        assert ("patch_gather_nhwc_tma" in e.name) == tma, (dtype, c, k, e.name)
-        assert "patch_gather_nhwc" in e.name and ("bfloat16" if dtype == "bf16" else "half") in e.name, e.name
+        assert ("patch_gather_nhwc_tma" in n) == tma, (dtype, c, k, n)
+        assert "patch_gather_nhwc" in n and ("bfloat16" if dtype == "bf16" else "half") in n, n
 
 
 @DTYPES
@@ -109,14 +112,13 @@ def test_pinned_host_nchw_reader_of_16bit_map(engine, dtype, c, k, pad, stride):
     dev = engine.device
     H, B, nb = 11, 3, 4
     m16 = _map16((nb * B, c, H, H), dtype, 500 + c, dev)
-    host = torch.empty(m16.shape, dtype=m16.dtype, pin_memory=True)
-    host.copy_(m16)
+    host = GC.pinned(m16)
     rx, ry, P = _points(nb, (H + 2 * pad - k) // stride + 1, dev)
     for relu in (False, True):
         want = engine.patch_gather(m16.float(), rx, ry, B, P, k, pad, stride, relu=relu)
         got = engine.patch_gather(host, rx, ry, B, P, k, pad, stride, relu=relu)
         torch.cuda.synchronize()
-        _assert_same_bits(got, want)
+        GC.assert_same_bits(got, want)
 
 
 @DTYPES
@@ -126,15 +128,14 @@ def test_point_gather_of_16bit_map_equals_gather_of_widened_map(engine, dtype, n
     H, B, nb = 9, 3, 4
     m16 = _map16((nb * B, n, H, H), dtype, 900 + n, dev)
     rx, ry, P = _points(nb, H, dev)
-    host = torch.empty(m16.shape, dtype=m16.dtype, pin_memory=True)
-    host.copy_(m16)
+    host = GC.pinned(m16)
     want = engine.point_gather(m16.float(), rx, ry, B, P)
-    _assert_same_bits(engine.point_gather(m16, rx, ry, B, P), want)
-    _assert_same_bits(engine.point_gather(host, rx, ry, B, P), want)
+    GC.assert_same_bits(engine.point_gather(m16, rx, ry, B, P), want)
+    GC.assert_same_bits(engine.point_gather(host, rx, ry, B, P), want)
     torch.cuda.synchronize()
     l16, l32 = m16.permute(0, 2, 3, 1).contiguous(), m16.float().permute(0, 2, 3, 1).contiguous()
-    _assert_same_bits(engine.point_gather(l16, rx, ry, B, P, layout="nhwc"),
-                      engine.point_gather(l32, rx, ry, B, P, layout="nhwc"))
+    GC.assert_same_bits(engine.point_gather(l16, rx, ry, B, P, layout="nhwc"),
+                        engine.point_gather(l32, rx, ry, B, P, layout="nhwc"))
 
 
 # ---------------------------------------------------------------------------- end to end

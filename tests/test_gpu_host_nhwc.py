@@ -4,43 +4,15 @@ the HBM NHWC path refuses, and leave the host-resident pruning pipeline's result
 import numpy as np
 import pytest
 
+import gather_checks as GC
+
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
 
-_T = {"fp32": torch.float32, "bf16": torch.bfloat16, "fp16": torch.float16}
-DTYPES = pytest.mark.parametrize("dtype", list(_T))
+DTYPES = pytest.mark.parametrize("dtype", list(GC.FMAP_DTYPES))
 # (k, pad, stride)
 WINDOWS = [(1, 0, 1), (1, 0, 2), (3, 1, 1), (3, 1, 2), (3, 0, 1), (5, 2, 1), (5, 2, 2)]
 CHANNELS = [3, 5, 12, 16, 24, 64, 512, 2048]
-
-
-def _map(shape, dtype, seed, device):
-    """N(0,1) drawn in fp32 and rounded to dtype, with -0, +-inf, NaN and subnormals (of fp32, bf16 and fp16) seeded
-    in."""
-    g = torch.Generator(device=device)
-    g.manual_seed(seed)
-    fm = torch.randn(shape, generator=g, device=device)
-    flat = fm.view(-1)
-    specials = torch.tensor([-0.0, float("inf"), float("-inf"), float("nan"), 6e-8, -3e-6, 4e-5, 1e-39, -5e-39,
-                             1e-44], device=device)
-    idx = torch.randperm(flat.numel(), generator=g, device=device)[:max(len(specials), flat.numel() // 40)]
-    flat[idx] = specials[torch.arange(idx.numel(), device=device) % len(specials)]
-    return fm.to(_T[dtype])
-
-
-def _pinned(t):
-    h = torch.empty(t.shape, dtype=t.dtype, pin_memory=True)
-    h.copy_(t)
-    return h
-
-
-def _assert_same_bits(got, want):
-    """Bit equality (so -0 and +0 differ); NaN positions compared separately, their payloads not."""
-    assert got.dtype == want.dtype == torch.float32 and got.shape == want.shape
-    ng, nw = torch.isnan(got), torch.isnan(want)
-    assert torch.equal(ng, nw)
-    z = torch.zeros_like(got)
-    assert torch.equal(torch.where(ng, z, got).view(torch.int32), torch.where(nw, z, want).view(torch.int32))
 
 
 def _points(nb, Ho, device):
@@ -59,17 +31,17 @@ def _points(nb, Ho, device):
 def test_host_nhwc_gather_equals_hbm_gathers(engine, dtype, c, k, pad, stride):
     dev = engine.device
     H, B, nb = 9, 3, 4
-    nchw = _map((nb * B, c, H, H), dtype, c * 31 + k * 7 + stride + pad, dev)
+    nchw = GC.special_map((nb * B, c, H, H), dtype, c * 31 + k * 7 + stride + pad, dev)
     nhwc = nchw.permute(0, 2, 3, 1).contiguous()
-    host = _pinned(nhwc)
+    host = GC.pinned(nhwc)
     rx, ry, P = _points(nb, (H + 2 * pad - k) // stride + 1, dev)
     for relu in (False, True):
         a = engine.patch_gather(nchw, rx, ry, B, P, k, pad, stride, relu=relu)
         b = engine.patch_gather(nhwc, rx, ry, B, P, k, pad, stride, relu=relu, layout="nhwc")
         got = engine.patch_gather(host, rx, ry, B, P, k, pad, stride, relu=relu, layout="nhwc")
         torch.cuda.synchronize()
-        _assert_same_bits(b, a)
-        _assert_same_bits(got, b)
+        GC.assert_same_bits(b, a)
+        GC.assert_same_bits(got, b)
         if relu:
             assert not bool(torch.isnan(got).any())  # fmaxf(NaN, 0) = 0, as in the HBM kernels
 
@@ -89,21 +61,21 @@ def test_host_nhwc_gather_at_conv4_2_size(engine, dtype):
     dev = engine.device
     g = torch.Generator(device=dev)
     g.manual_seed(5)
-    nhwc = torch.randn((s.nbatch * s.B, s.H, s.W, s.c), generator=g, device=dev).to(_T[dtype])
-    host = _pinned(nhwc)
+    nhwc = torch.randn((s.nbatch * s.B, s.H, s.W, s.c), generator=g, device=dev).to(GC.FMAP_DTYPES[dtype])
+    host = GC.pinned(nhwc)
     r = np.random.RandomState(3)
     rx = torch.as_tensor(r.randint(0, s.Ho, (s.nbatch, s.P)).astype(np.int32), device=dev)
     ry = torch.as_tensor(r.randint(0, s.Ho, (s.nbatch, s.P)).astype(np.int32), device=dev)
     want = engine.patch_gather(nhwc, rx, ry, s.B, s.P, s.k, s.pad, s.stride, layout="nhwc")
     got = engine.patch_gather(host, rx, ry, s.B, s.P, s.k, s.pad, s.stride, layout="nhwc")
     torch.cuda.synchronize()
-    _assert_same_bits(got, want)
+    GC.assert_same_bits(got, want)
     del got
     wide = torch.full((s.N, s.K + 40), 7.0, device=dev)
     out = wide[:, 8:8 + s.K]
     engine.patch_gather(host, rx, ry, s.B, s.P, s.k, s.pad, s.stride, layout="nhwc", out=out)
     torch.cuda.synchronize()
-    _assert_same_bits(out.contiguous(), want)
+    GC.assert_same_bits(out.contiguous(), want)
     assert bool((wide[:, :8] == 7.0).all()) and bool((wide[:, 8 + s.K:] == 7.0).all())
 
 
@@ -121,9 +93,9 @@ def test_host_nhwc_reader_is_what_runs(engine):
     H, B, nb = 7, 2, 2
     rx, ry, P = _points(nb, H, dev)
     runs = []
-    for dtype in _T:
+    for dtype in GC.FMAP_DTYPES:
         for c, k in PATH_SHAPES:
-            host = _pinned(_map((nb * B, H, H, c), dtype, c + k, dev))
+            host = GC.pinned(GC.special_map((nb * B, H, H, c), dtype, c + k, dev))
             out = engine.patch_gather(host, rx, ry, B, P, k, k // 2, 1, layout="nhwc")  # warm-up (module load)
             runs.append((dtype, c, k, host, out))
     torch.cuda.synchronize()
@@ -136,7 +108,7 @@ def test_host_nhwc_reader_is_what_runs(engine):
     kernels = [e.name for e in prof.events() if "patch_gather" in e.name and e.device_type.name == "CUDA"]
     assert kernels and all("patch_gather_nhwc_host" in n for n in kernels), sorted(set(kernels))
     ctype = {"fp32": "float", "bf16": "bfloat16", "fp16": "half"}
-    for dtype in _T:
+    for dtype in GC.FMAP_DTYPES:
         seen = sum(1 for n in kernels if "%s>" % ctype[dtype] in n or "%s >" % ctype[dtype] in n)
         want = REPEAT * sum(1 for r in runs if r[0] == dtype)
         assert want - LOST <= seen <= want, (dtype, seen, want, sorted(set(kernels)))
@@ -147,7 +119,7 @@ def test_oversized_window_on_nhwc_host_map_is_refused(engine):
     ffi, lib = engine.ffi, engine.lib
     dev = engine.device
     H, B, nb, k = 13, 2, 1, 11
-    host = _pinned(torch.zeros((nb * B, H, H, 3), device=dev))
+    host = GC.pinned(torch.zeros((nb * B, H, H, 3), device=dev))
     rx = torch.zeros((nb, 1), dtype=torch.int32, device=dev)
     X = torch.empty((nb * B, 3 * k * k), device=dev)
     rc = lib.cp_patch_gather_typed(engine.h, ffi.cast("const void*", host.data_ptr()), lib.CP_F32, nb, B, 3, H, H, 1,
@@ -177,7 +149,7 @@ def test_host_resident_pipeline_on_nhwc_maps_equals_nchw_maps(dtype, policy):
 
     eng = cpb200.Engine(nstreams=4)
     shapes = _shapes()
-    dt = None if dtype == "fp32" else _T[dtype]
+    dt = None if dtype == "fp32" else GC.FMAP_DTYPES[dtype]
     dn = [cpb200.synth.make_problem_device(s, 70 + i, eng, pinned_host=True, dtype=dt) for i, s in enumerate(shapes)]
     dh = [cpb200.synth.make_problem_device(s, 70 + i, eng, pinned_host=True, dtype=dt, host_layout="nhwc")
           for i, s in enumerate(shapes)]

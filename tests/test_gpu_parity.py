@@ -11,15 +11,12 @@ import pytest
 
 import cases
 import cp_oracle as O
+import gather_checks as GC
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
 
 W_TOL = 1e-4  # north_star tolerance on reconstructed weights (relative Frobenius)
-
-
-def _rel(a, b):
-    return np.linalg.norm(a - b) / np.linalg.norm(b)
 
 
 @pytest.mark.parametrize("mode", [0, 1], ids=["fp64", "3xtf32"])
@@ -45,11 +42,11 @@ def test_dictionary_matches_reference_golden(engine, golden_dir, name, mode):
     assert after == int(g["rng_after"])  # consumed the same global RNG draws as the reference
     assert cfgs.alpha == float(g["alpha_final"])
     assert W.dtype == np.float64 and W.shape == g["W"].shape
-    assert _rel(W, g["W"]) <= W_TOL
+    assert GC.rel(W, g["W"]) <= W_TOL
     # what the two arithmetic modes actually deliver; the near-collinear case (cond of the centred Gram 2e10) is
     # limited by the normal equations in fp64, cond * 2e-16
     tight = spec.get("w_tol", 1e-7 if mode == 0 else 2e-5)
-    assert _rel(W, g["W"]) <= tight
+    assert GC.rel(W, g["W"]) <= tight
     assert np.abs(B - g["B"]).max() <= tight * max(1.0, np.abs(g["B"]).max())
 
 
@@ -65,7 +62,7 @@ def test_dictionary_accepts_cuda_tensors(engine, golden_dir):
     np.random.seed(spec["np_seed"])
     idxs, W, B = decompose.dictionary(torch.as_tensor(X, device=engine.device), torch.as_tensor(W2, device=engine.device),
                                       torch.as_tensor(Y, device=engine.device), rank=spec["rank"])
-    assert np.array_equal(idxs, g["idxs"]) and _rel(W, g["W"]) <= 1e-7
+    assert np.array_equal(idxs, g["idxs"]) and GC.rel(W, g["W"]) <= 1e-7
 
 
 def test_fc_kernel_matches_oracle(engine):
@@ -78,7 +75,7 @@ def test_fc_kernel_matches_oracle(engine):
     Y = (X @ r.standard_normal((250, 20)) + 0.1 * r.standard_normal((900, 20)))
     coef, icpt = decompose.fc_kernel(X.astype(np.float64), Y)
     rc, ri = O.fc_kernel(X.astype(np.float64), Y)
-    assert _rel(coef, rc) <= 1e-8 and np.abs(icpt - ri).max() <= 1e-8
+    assert GC.rel(coef, rc) <= 1e-8 and np.abs(icpt - ri).max() <= 1e-8
     with pytest.raises(AssertionError):
         decompose.fc_kernel(X[None], Y)  # reference asserts 2-D input (decompose.py:641)
 
@@ -136,7 +133,7 @@ def test_net_methods_match_reference_golden(engine, golden_dir, name):
         idxs, W, B = net.dictionary_kernel(spec["xy"][0], None, int(g["dk_dprime"]), spec["xy"][1], None)
         assert np.array_equal(idxs, g["dk_idxs"])
         assert cfgs.alpha == float(g["dk_alpha"])
-        assert _rel(W, g["dk_W"]) <= 1e-7 and np.abs(B - g["dk_B"]).max() <= 1e-7
+        assert GC.rel(W, g["dk_W"]) <= 1e-7 and np.abs(B - g["dk_B"]).max() <= 1e-7
 
 
 def test_baseline_config1_mask_bit_compare(engine):
@@ -156,7 +153,7 @@ def test_baseline_config1_mask_bit_compare(engine):
     assert np.array_equal(idxs, oi)
     assert decompose.DictionaryInfo.last["probes"] == info["probes"]  # same alpha probes and counts
     assert cfgs.alpha == st.alpha
-    assert _rel(W, oW) <= W_TOL and np.abs(B - oB).max() <= W_TOL
+    assert GC.rel(W, oW) <= W_TOL and np.abs(B - oB).max() <= W_TOL
 
 
 @pytest.mark.parametrize("mode", [0, 1], ids=["fp64", "3xtf32"])
@@ -228,36 +225,15 @@ def test_resnet50_bottleneck_problem_vs_oracle(engine, name):
     forward = lambda b: {"x": fm[b * s.B:(b + 1) * s.B]}  # noqa: E731
     st_ = O.DictState(alpha=1e-3)
     info = {}
-
-    class _Seeds:  # the oracle draws its CD seeds from an RNG object: feed it the device's seed list
-        def __init__(self, seeds):
-            self.seeds, self.i = list(seeds), 0
-
-        def randint(self, lo, hi):
-            v = self.seeds[self.i]
-            self.i += 1
-            return v
-
-    import cp_oracle
-
-    orig = cp_oracle.LassoCD.__init__
-
-    def patched(self, alpha, **kw):
-        orig(self, alpha, **kw)
-        self.rng = _Seeds(d["seeds"])
-
-    cp_oracle.LassoCD.__init__ = patched
-    try:
+    with GC.seeded_lasso(d["seeds"]):
         oi, oW, oB = O.dictionary_kernel(forward, "x", O.ConvSpec("y", "x", k, pad, st), d["W2"].cpu().numpy(),
                                          d["b2"].cpu().numpy(), d["feats"].cpu().numpy().astype(np.float64), pd, kept,
                                          state=st_, samples=d["samples"].cpu().numpy(), info=info)
-    finally:
-        cp_oracle.LassoCD.__init__ = orig
     assert np.array_equal(res.idxs, oi)
     if kept != c:
         assert res.alpha == st_.alpha and res.nprobe == len(info["probes"])
     W = res.W.cpu().numpy().reshape(oW.shape)
-    assert _rel(W, oW) <= W_TOL and np.abs(res.b.cpu().numpy() - oB).max() <= W_TOL
+    assert GC.rel(W, oW) <= W_TOL and np.abs(res.b.cpu().numpy() - oB).max() <= W_TOL
 
 
 @pytest.mark.parametrize("policy", [True, "zc", "copy"])

@@ -5,6 +5,8 @@ import types
 import numpy as np
 import pytest
 
+import gather_checks as GC
+
 torch = pytest.importorskip("torch")
 
 
@@ -66,12 +68,6 @@ def test_nhwc_line_model_at_vgg16_shapes():
             assert pruner.zero_copy_lines(s, es, "nhwc") < pruner.zero_copy_lines(s, es, "nchw")
 
 
-def _all_shapes():
-    import cpb200
-
-    return cpb200.synth.vgg16_layers() + cpb200.synth.resnet50_layers()
-
-
 def _maps(shapes, dtype, host_layout=None):
     out = []
     for s in shapes:
@@ -93,7 +89,7 @@ def default_rule(monkeypatch):
 def test_plan_of_nhwc_maps_uses_nhwc_lines_and_their_rate(default_rule, dtype):
     from cpb200 import pruner
 
-    shapes = _all_shapes()
+    shapes = GC.all_shapes()
     datas = _maps(shapes, dtype, "nhwc")
     es = torch.empty((), dtype=dtype).element_size()
     plan = pruner.h2d_plan(shapes, datas, True)
@@ -111,7 +107,7 @@ def test_maps_without_host_layout_keep_todays_plan(default_rule, dtype):
     """No host_layout key: NCHW lines at ZC_LINES_PER_S, exactly the plan an explicit 'nchw' gets."""
     from cpb200 import pruner
 
-    shapes = _all_shapes()
+    shapes = GC.all_shapes()
     plain = _maps(shapes, dtype)
     es = torch.empty((), dtype=dtype).element_size()
     want = []
