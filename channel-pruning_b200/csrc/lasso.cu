@@ -13,6 +13,9 @@
 // the model rounds separately is issued with an explicit *_rn intrinsic (no FMA
 // contraction), the gap reductions run in the model's "warp order", the division is
 // correctly rounded, and the random coordinate order comes from the same 32-bit xorshift.
+// Q need not be bitwise symmetric (cp_lasso_build sums the products of Q[a][b] and of Q[b][a] in different orders):
+// every entry is read where the model reads it -- the update of coordinate j uses row j, the screening's correction
+// of an evicted j uses row j.
 //
 // Coordinate descent is one long serial dependency chain (each coordinate update needs the
 // previous one), so the search is latency bound and is organised as ONE warp-specialised CTA
@@ -25,7 +28,7 @@
 //                  (DMUL / DADD), stream the rows of Q from L2 into a register ring several steps ahead, and
 //                  publish the Qw entry the chain warp will need LAG+1 steps later
 //   packager warp  per-step operands of the chain (q_j, Q_jj, 1/Q_jj, the LAG entries
-//                  Q[j_s][j_{s-i}]) gathered 32 steps at a time, lane-parallel
+//                  Q[j_{s-i}][j_s]) gathered 32 steps at a time, lane-parallel
 //   sequencer warp the xorshift stream of the NEXT sweep (it does not depend on the active set)
 // Hand-offs are release/acquire counters in shared memory (bounded spins: a protocol bug traps
 // instead of hanging); CTA barriers only at sweep boundaries.
@@ -455,7 +458,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) lasso_select_kernel(const Selec
                     CH_STAMP(s, 2);
                     double x = xv;
 #pragma unroll
-                    for (int k = LAG; k >= 1; --k)  // oldest delta first: delta_{s-k} * Q[j_s][j_{s-k}]
+                    for (int k = LAG; k >= 1; --k)  // oldest delta first: delta_{s-k} * Q[j_{s-k}][j_s]
                         x = __dadd_rn(x, __dmul_rn(D[(i + 16 * LAG - k) % LAG], P[cur][2 + k]));
                     double delta, aw, w_new;
                     cd_update(P[cur][0], P[cur][1], P[cur][2], x, WJ[cur], l1, delta, aw, w_new);
@@ -583,10 +586,11 @@ __global__ void __launch_bounds__(WS_THREADS, 1) lasso_select_kernel(const Selec
                 if (s < n_active) {
                     const uint32_t j = jz[s];
                     const double d = dg[j];
-                    const double *qrow = Q + (int64_t)j * ldq;
+                    // Q[j_{s-i}][j]: step s-i added its delta times row j_{s-i} to Qw (Q need not be bitwise symmetric)
                     double rr[5];
 #pragma unroll
-                    for (int i = 1; i <= 5; ++i) rr[i - 1] = (i <= LAG && s >= i) ? __ldg(qrow + jz[s - i]) : 0.0;
+                    for (int i = 1; i <= 5; ++i)
+                        rr[i - 1] = (i <= LAG && s >= i) ? __ldg(Q + (int64_t)jz[s - i] * ldq + j) : 0.0;
                     double *o = pk + (s & (QR - 1)) * 8;
                     *reinterpret_cast<double2 *>(o) = make_double2(qv[j], d);
                     *reinterpret_cast<double2 *>(o + 2) = make_double2(d != 0.0 ? __drcp_rn(d) : 0.0, rr[0]);

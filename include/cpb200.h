@@ -254,7 +254,8 @@ int cp_lasso_build(cp_handle_t h, const double *Gs, const double *Bs, const doub
  * xorshift seeded per fit, warm start, tol / duality-gap stopping rule, gap-safe
  * screening), evaluated in Gram arithmetic, fp64, in ONE launch (one warp: the search is a
  * serial dependency chain).  Q: c x ldq row-major, ldq even, base 16-byte aligned, any
- * padding column zero.
+ * padding column zero; it need not be bitwise symmetric (cp_lasso_build's is not): the update
+ * of coordinate j reads row j, as the model oracle/cd_oracle.c:cp_enet_cd_gram does.
  *
  *   right0        : cfgs.alpha on entry (lib/decompose.py:491)
  *   rank, lbound, rbound : target count and acceptance window (:492-501)

@@ -158,7 +158,8 @@ done:
 }
 
 /*
- * Same control flow, Gram arithmetic.  Q (nf x nf, row-major, leading dimension ldq, symmetric)
+ * Same control flow, Gram arithmetic.  Q (nf x nf, row-major, leading dimension ldq, symmetric up
+ * to rounding: the update of coordinate j reads row j only)
  * = X'X, q = X'y, y_norm2 = y'y (all of centred data).  This is, operation for operation, what
  * the CUDA kernel cp_lasso_select (csrc/lasso.cu) executes:
  *   - Qw = Q w is CARRIED between fits (in/out argument; all zeros with w = 0 before the first
