@@ -47,6 +47,39 @@ struct cp_window {
     int kt, kh, kw, pad_t, pad_h, pad_w, stride_t, stride_h, stride_w, dil_t, dil_h, dil_w;
 };
 
+// The input transform of a consumer (cp_patch_gather_act): an activation act (CP_ACT_*, slope: LeakyReLU's negative
+// slope) after an optional per-channel affine (scale[a], shift[a]), the producer's eval-mode BatchNorm folded; either
+// pointer may be NULL (scale 1, shift 0).
+struct cp_xform {
+    int act;
+    float slope;
+    const float *scale, *shift;
+};
+
+// The transform of an in-map tap on (global) channel a, v the widened value.  Each operation is rounded in fp32 (no
+// FMA contraction); without an affine no arithmetic touches v, so -0 stays -0 under the identity.  Taps outside the
+// map are never passed here: they are +0 whatever the transform (the consumer's zero padding pads its
+// post-activation input).  SiLU is v / (1 + expf(-v)) with the accurate expf; below -64, where expf(-v) heads for
+// overflow, the same value as (v e) e with e = expf(v / 2), which keeps the result within 4 ulp down to the
+// subnormals.
+__device__ __forceinline__ float cp_xform_apply(const cp_xform &f, float v, int a) {
+    if (f.scale) v = __fmul_rn(v, __ldg(f.scale + a));
+    if (f.shift) v = __fadd_rn(v, __ldg(f.shift + a));
+    switch (f.act) {
+        case CP_ACT_RELU: return fmaxf(v, 0.f);
+        case CP_ACT_RELU6: return fminf(fmaxf(v, 0.f), 6.f);
+        case CP_ACT_LEAKY_RELU: return v > 0.f ? v : __fmul_rn(v, f.slope);
+        case CP_ACT_HARDSWISH: return __fdiv_rn(__fmul_rn(v, fminf(fmaxf(__fadd_rn(v, 3.f), 0.f), 6.f)), 6.f);
+        case CP_ACT_SILU:
+            if (v < -64.f) {
+                const float e = expf(0.5f * v);
+                return __fmul_rn(__fmul_rn(v, e), e);
+            }
+            return __fdiv_rn(v, __fadd_rn(1.f, expf(-v)));
+        default: return v;  // CP_ACT_IDENTITY
+    }
+}
+
 // One patch gather as an entry point hands it to a path (gather.cu, gather_host.cu, gather_tma.cu): nbatch*B images
 // of c x D x H x W, channels first (CP_LAYOUT_NCHW) or last (CP_LAYOUT_NHWC); randt NULL for a 2-D map (D = 1, t = 0).
 struct cp_patch_args {
@@ -59,6 +92,9 @@ struct cp_patch_args {
     float *X;
     int64_t ldx;
     cudaStream_t stream;
+    // cp_patch_gather_act: the input transform, applied by the paths' XFORM = true kernels (relu then unused)
+    bool fused = false;
+    cp_xform xf = {};
     int64_t rows() const { return (int64_t)nbatch * P * B; }
 };
 

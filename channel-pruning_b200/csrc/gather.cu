@@ -21,18 +21,22 @@
 // Element type of the map: fp32, bf16 or fp16 (template parameter T, fmap_types.cuh).  X and Y are fp32 in every
 // case; the ReLU is applied to the widened value with the fp32 kernel's expression, so -0, inf and NaN come out as the
 // fp32 kernel gives them for the widened map.
+// cp_patch_gather_act runs each path's XFORM = true instantiation: the consumer's input transform (cp_xform_apply,
+// fmap_types.cuh: a folded BatchNorm and an activation) on every in-map tap, +0 on the others.  The XFORM = false
+// instantiations are the relu-flag kernels of the other entries, unchanged.
 #include "common.cuh"
 #include "fmap_types.cuh"
 
 namespace {
 
-// KS > 0: a square, undilated KS x KS 2-D window known at compile time (1 and 3); KS = 0: any window of g
-template <int KS, bool DEPTH, typename T>
+// KS > 0: a square, undilated KS x KS 2-D window known at compile time (1 and 3); KS = 0: any window of g.
+// XFORM: the input transform xf on in-map taps (cp_patch_gather_act); otherwise the relu flag.
+template <int KS, bool DEPTH, bool XFORM, typename T>
 __device__ __forceinline__ void cfirst_body(const T *__restrict__ fmap, const int32_t *__restrict__ randt,
                                             const int32_t *__restrict__ randx,
                                             const int32_t *__restrict__ randy, float *__restrict__ X, int64_t ldx,
                                             int64_t rows, int B, int c, int D, int H, int W, int P, const cp_window &g,
-                                            int relu) {
+                                            int relu, const cp_xform &xf) {
     const int k = KS > 0 ? KS * KS : (DEPTH ? g.kt : 1) * g.kh * g.kw;  // taps
     const int K = c * k;
     // one CTA per output row when the map is in HBM; a small persistent grid strides over the rows when the
@@ -51,9 +55,11 @@ __device__ __forceinline__ void cfirst_body(const T *__restrict__ fmap, const in
             const int a = col / k;
             int tt, yy, xx;
             float v = 0.f;
-            if (cp_window_tap<DEPTH, KS>(g, col - a * k, t0, y0, x0, D, H, W, tt, yy, xx))
+            if (cp_window_tap<DEPTH, KS>(g, col - a * k, t0, y0, x0, D, H, W, tt, yy, xx)) {
                 v = cp_widen(__ldg(src + (DEPTH ? (((int64_t)a * D + tt) * H + yy) * W : ((int64_t)a * H + yy) * W) + xx));
-            if (relu) v = fmaxf(v, 0.f);
+                if (XFORM) v = cp_xform_apply(xf, v, a);
+            }
+            if (!XFORM && relu) v = fmaxf(v, 0.f);
             dst[col] = v;
         }
     }
@@ -64,14 +70,14 @@ __device__ __forceinline__ void cfirst_body(const T *__restrict__ fmap, const in
 #define CP_CFIRST_PARAMS                                                                                              \
     const T *__restrict__ fmap, const int32_t *__restrict__ randt, const int32_t *__restrict__ randx,                  \
         const int32_t *__restrict__ randy, float *__restrict__ X, int64_t ldx, int64_t rows, int B, int c, int D, int H, \
-        int W, int P, cp_window g, int relu
-template <int KS, typename T>
+        int W, int P, cp_window g, int relu, cp_xform xf
+template <int KS, typename T, bool XFORM = false>
 __global__ void __launch_bounds__(256) patch_gather_nchw(CP_CFIRST_PARAMS) {
-    cfirst_body<KS, false>(fmap, nullptr, randx, randy, X, ldx, rows, B, c, 1, H, W, P, g, relu);
+    cfirst_body<KS, false, XFORM>(fmap, nullptr, randx, randy, X, ldx, rows, B, c, 1, H, W, P, g, relu, xf);
 }
-template <typename T>
+template <typename T, bool XFORM = false>
 __global__ void __launch_bounds__(256) patch_gather_ncdhw(CP_CFIRST_PARAMS) {
-    cfirst_body<0, true>(fmap, randt, randx, randy, X, ldx, rows, B, c, D, H, W, P, g, relu);
+    cfirst_body<0, true, XFORM>(fmap, randt, randx, randy, X, ldx, rows, B, c, D, H, W, P, g, relu, xf);
 }
 
 constexpr int64_t CP_HOST_GATHER_CTAS = 64;  // grid of the in-place (zero-copy) channels-first reader
@@ -79,11 +85,11 @@ constexpr int CLAST_TILE_FLOATS = 12 * 1024;  // shared-memory tile of the chann
 
 // grid (rows, channel tiles); the tile is [taps][ct_tile + 1] floats, ct_tile channels (ct_tile + 1: the transposed
 // read is conflict-free)
-template <bool DEPTH, typename T>
+template <bool DEPTH, bool XFORM, typename T>
 __device__ __forceinline__ void clast_body(const T *__restrict__ fmap, const int32_t *__restrict__ randt,
                                            const int32_t *__restrict__ randx, const int32_t *__restrict__ randy,
                                            float *__restrict__ X, int64_t ldx, int B, int c, int D, int H, int W, int P,
-                                           const cp_window &g, int ct_tile, int relu) {
+                                           const cp_window &g, int ct_tile, int relu, const cp_xform &xf) {
     extern __shared__ float tile[];
     const int k = (DEPTH ? g.kt : 1) * g.kh * g.kw;
     const int64_t r = blockIdx.x;
@@ -101,9 +107,11 @@ __device__ __forceinline__ void clast_body(const T *__restrict__ fmap, const int
         const int a = e - p * ct;
         int tt, yy, xx;
         float v = 0.f;
-        if (cp_window_tap<DEPTH>(g, p, t0, y0, x0, D, H, W, tt, yy, xx))
+        if (cp_window_tap<DEPTH>(g, p, t0, y0, x0, D, H, W, tt, yy, xx)) {
             v = cp_widen(__ldg(src + cp_pixel<DEPTH>(tt, yy, xx, H, W) * c + a0 + a));
-        if (relu) v = fmaxf(v, 0.f);
+            if (XFORM) v = cp_xform_apply(xf, v, a0 + a);
+        }
+        if (!XFORM && relu) v = fmaxf(v, 0.f);
         tile[p * (ct_tile + 1) + a] = v;
     }
     __syncthreads();
@@ -118,14 +126,14 @@ __device__ __forceinline__ void clast_body(const T *__restrict__ fmap, const int
 #define CP_CLAST_PARAMS                                                                                               \
     const T *__restrict__ fmap, const int32_t *__restrict__ randt, const int32_t *__restrict__ randx,                  \
         const int32_t *__restrict__ randy, float *__restrict__ X, int64_t ldx, int B, int c, int D, int H, int W, int P, \
-        cp_window g, int ct_tile, int relu
-template <typename T>
+        cp_window g, int ct_tile, int relu, cp_xform xf
+template <typename T, bool XFORM = false>
 __global__ void __launch_bounds__(256) patch_gather_nhwc(CP_CLAST_PARAMS) {
-    clast_body<false>(fmap, nullptr, randx, randy, X, ldx, B, c, 1, H, W, P, g, ct_tile, relu);
+    clast_body<false, XFORM>(fmap, nullptr, randx, randy, X, ldx, B, c, 1, H, W, P, g, ct_tile, relu, xf);
 }
-template <typename T>
+template <typename T, bool XFORM = false>
 __global__ void __launch_bounds__(256) patch_gather_ndhwc(CP_CLAST_PARAMS) {
-    clast_body<true>(fmap, randt, randx, randy, X, ldx, B, c, D, H, W, P, g, ct_tile, relu);
+    clast_body<true, XFORM>(fmap, randt, randx, randy, X, ldx, B, c, D, H, W, P, g, ct_tile, relu, xf);
 }
 
 // randt NULL: a 2-D map (t = 0)
@@ -161,7 +169,7 @@ int cp_patch_gather_host(const cp_patch_args &a);
 // gather_tr.cu: the gathers of transposed convolutions, every layout, from HBM or (host_src) pinned host memory
 int cp_patch_gather_tr(const cp_patch_args &a, bool host_src);
 
-template <typename T>
+template <typename T, bool XFORM>
 static void launch_patch_gather_simt(const cp_patch_args &a, bool host_src) {
     const cp_window &g = a.g;
     const T *fmap = (const T *)a.fmap;
@@ -170,21 +178,21 @@ static void launch_patch_gather_simt(const cp_patch_args &a, bool host_src) {
     if (a.layout == CP_LAYOUT_NCHW) {
         const int64_t ncta = host_src ? (rows < CP_HOST_GATHER_CTAS ? rows : CP_HOST_GATHER_CTAS) : rows;
         const bool square = !depth && g.kh == g.kw && g.dil_h == 1 && g.dil_w == 1;
-        auto kern = depth                   ? patch_gather_ncdhw<T>
-                    : square && g.kh == 3 ? patch_gather_nchw<3, T>
-                    : square && g.kh == 1 ? patch_gather_nchw<1, T>
-                                          : patch_gather_nchw<0, T>;
+        auto kern = depth                   ? patch_gather_ncdhw<T, XFORM>
+                    : square && g.kh == 3 ? patch_gather_nchw<3, T, XFORM>
+                    : square && g.kh == 1 ? patch_gather_nchw<1, T, XFORM>
+                                          : patch_gather_nchw<0, T, XFORM>;
         kern<<<(unsigned)ncta, 256, 0, a.stream>>>(fmap, a.randt, a.randx, a.randy, a.X, a.ldx, rows, a.B, a.c, a.D,
-                                                   a.H, a.W, a.P, g, a.relu);
+                                                   a.H, a.W, a.P, g, a.relu, a.xf);
     } else {
         // channels per tile: up to 128, fewer for windows over 95 taps so the tile stays within 48 KB
         const int k = g.kt * g.kh * g.kw;
         const int ct_tile = CLAST_TILE_FLOATS / k - 1 > 128 ? 128 : CLAST_TILE_FLOATS / k - 1;
         const size_t smem = (size_t)k * (ct_tile + 1) * sizeof(float);
         dim3 grid((unsigned)rows, (unsigned)cp_cdiv(a.c, ct_tile));
-        auto kern = depth ? patch_gather_ndhwc<T> : patch_gather_nhwc<T>;
+        auto kern = depth ? patch_gather_ndhwc<T, XFORM> : patch_gather_nhwc<T, XFORM>;
         kern<<<grid, 256, smem, a.stream>>>(fmap, a.randt, a.randx, a.randy, a.X, a.ldx, a.B, a.c, a.D, a.H, a.W, a.P,
-                                            g, ct_tile, a.relu);
+                                            g, ct_tile, a.relu, a.xf);
     }
 }
 
@@ -272,7 +280,12 @@ static int cp_patch_gather_any(const cp_gather_limits &L, cp_handle_t h, const c
         CP_REQUIRE(!L.max_simt_taps || taps <= L.max_simt_taps, "%s: kernel_size %s too large for the NHWC tile",
                    L.name, cp_axes(s, L.d3, "x", g.kt, g.kh, g.kw));
     }
-    cp_with_fmap_type(a.dtype, [&](auto z) { launch_patch_gather_simt<decltype(z)>(a, kind == CP_MEM_HOST); });
+    cp_with_fmap_type(a.dtype, [&](auto z) {
+        if (a.fused)
+            launch_patch_gather_simt<decltype(z), true>(a, kind == CP_MEM_HOST);
+        else
+            launch_patch_gather_simt<decltype(z), false>(a, kind == CP_MEM_HOST);
+    });
     CP_CHECK_LAUNCH();
     return CP_OK;
 }
@@ -334,6 +347,31 @@ extern "C" int cp_patch_gather_conv_transpose3d(cp_handle_t h, const void *fmap,
     return cp_patch_gather_any(CP_GATHER_TR_3D, h,
                                {CP_GATHER_TR_3D.name, fmap, fmap_dtype, layout, nbatch, B, c, D, H, W, P, randt, randx,
                                 randy, g, relu, X_out, ldx, (cudaStream_t)stream});
+}
+
+extern "C" int cp_patch_gather_act(cp_handle_t h, const void *fmap, int fmap_dtype, int nbatch, int B, int c, int D,
+                                   int H, int W, int layout, const int32_t *randt, const int32_t *randx,
+                                   const int32_t *randy, int P, int kt, int kh, int kw, int pad_t, int pad_h,
+                                   int pad_w, int stride_t, int stride_h, int stride_w, int dil_t, int dil_h,
+                                   int dil_w, int transposed, int act, float act_param, const float *in_scale,
+                                   const float *in_shift, float *X_out, int64_t ldx, cp_stream_t stream) {
+    const char *nm = "cp_patch_gather_act";
+    const bool d3 = randt != nullptr;
+    const cp_gather_limits &L0 = transposed ? (d3 ? CP_GATHER_TR_3D : CP_GATHER_TR_2D) : (d3 ? CP_GATHER_3D : CP_GATHER_2D);
+    CP_REQUIRE(act >= CP_ACT_IDENTITY && act <= CP_ACT_SILU, "%s: unknown act %d", nm, act);
+    CP_REQUIRE(isfinite(act_param), "%s: act_param must be finite", nm);
+    CP_REQUIRE(d3 || (D == 1 && kt == 1 && pad_t == 0 && stride_t == 1 && dil_t == 1),
+               "%s: a 2-D gather (randt NULL) takes D = 1, kt = 1, pad_t = 0, stride_t = dil_t = 1", nm);
+    CP_REQUIRE(!in_scale || cp_pointer_kind(in_scale) == CP_MEM_DEVICE, "%s: in_scale is not in device memory", nm);
+    CP_REQUIRE(!in_shift || cp_pointer_kind(in_shift) == CP_MEM_DEVICE, "%s: in_shift is not in device memory", nm);
+    cp_gather_limits L = L0;
+    L.name = nm;
+    cp_patch_args a{nm, fmap, fmap_dtype, layout, nbatch, B, c, D, H, W, P, randt, randx, randy,
+                    cp_window{kt, kh, kw, pad_t, pad_h, pad_w, stride_t, stride_h, stride_w, dil_t, dil_h, dil_w},
+                    0, X_out, ldx, (cudaStream_t)stream};
+    a.fused = true;
+    a.xf = cp_xform{act, act_param, in_scale, in_shift};
+    return cp_patch_gather_any(L, h, a);
 }
 
 // d3: the 3-D entry (randt required, D from the caller); otherwise D = 1 and randt NULL

@@ -13,7 +13,8 @@
 // layers' searches and Grams, which need the SMs.
 // Maps whose channel stride or base address is not a multiple of 16 bytes (c = 3, 5, 12 in fp32; odd c in 16 bit)
 // take plain element loads into the same stages: correct for every c, not tuned.
-// The output is bit for bit that of the HBM NHWC kernels: zero outside the map, cp_widen, then fmaxf for the ReLU.
+// The output is bit for bit that of the HBM NHWC kernels: zero outside the map, cp_widen, then fmaxf for the ReLU
+// (XFORM = true: the input transform of cp_patch_gather_act instead).
 // NDHWC maps (Conv3d windows, DEPTH = true) take kt*kh*kw taps per unit: each (u, i) row of an undilated window is
 // again one contiguous run of kw*c elements.
 #include "common.cuh"
@@ -73,11 +74,12 @@ __device__ __forceinline__ void host_fetch(const T *__restrict__ fmap, const int
     }
 }
 
-// Writes unit u from its stage: column a*taps + p of the chunk, zero for taps outside the map.
-template <bool DEPTH, typename T>
+// Writes unit u from its stage: column a*taps + p of the chunk, zero for taps outside the map.  XFORM: the input
+// transform xf on in-map taps; otherwise the relu flag.
+template <bool DEPTH, bool XFORM, typename T>
 __device__ __forceinline__ void host_store(const int32_t *__restrict__ randx, const int32_t *__restrict__ randy,
                                            float *__restrict__ X, int64_t ldx, const HostGeom &g, int64_t u,
-                                           const unsigned char *stage, int relu) {
+                                           const unsigned char *stage, int relu, const cp_xform &xf) {
     const int64_t r = u / g.nchunk;
     const int a0 = (int)(u - r * g.nchunk) * g.ct;
     const int ct = min(g.ct, g.c - a0);
@@ -91,18 +93,20 @@ __device__ __forceinline__ void host_store(const int32_t *__restrict__ randx, co
     for (int e = threadIdx.x; e < k * ct; e += blockDim.x) {
         const int a = e / k, p = e - a * k;
         float v = 0.f;
-        if (cp_window_tap<DEPTH>(g.w, p, t0, y0, x0, g.D, g.H, g.W, tt, yy, xx))
+        if (cp_window_tap<DEPTH>(g.w, p, t0, y0, x0, g.D, g.H, g.W, tt, yy, xx)) {
             v = cp_widen(reinterpret_cast<const T *>(stage + p * g.tap)[a]);
-        if (relu) v = fmaxf(v, 0.f);
+            if (XFORM) v = cp_xform_apply(xf, v, a0 + a);
+        }
+        if (!XFORM && relu) v = fmaxf(v, 0.f);
         dst[e] = v;
     }
 }
 
 // NS stages: unit u + i * gridDim.x is copied into stage (it + i) % NS while unit u is stored.
-template <int NS, bool DEPTH, typename T>
+template <int NS, bool DEPTH, bool XFORM, typename T>
 __device__ __forceinline__ void host_reader_body(const T *__restrict__ fmap, const int32_t *__restrict__ randx,
                                                  const int32_t *__restrict__ randy, float *__restrict__ X, int64_t ldx,
-                                                 int64_t units, const HostGeom &g, int relu) {
+                                                 int64_t units, const HostGeom &g, int relu, const cp_xform &xf) {
     extern __shared__ __align__(16) unsigned char nh_smem[];
     const int64_t step = gridDim.x;
 #pragma unroll
@@ -118,26 +122,27 @@ __device__ __forceinline__ void host_reader_body(const T *__restrict__ fmap, con
         asm volatile("cp.async.commit_group;" ::: "memory");
         asm volatile("cp.async.wait_group %0;" ::"n"(NS - 1) : "memory");  // unit u's copies have landed
         __syncthreads();
-        host_store<DEPTH, T>(randx, randy, X, ldx, g, u, nh_smem + (it % NS) * g.stage, relu);
+        host_store<DEPTH, XFORM, T>(randx, randy, X, ldx, g, u, nh_smem + (it % NS) * g.stage, relu, xf);
         __syncthreads();  // the stage is refilled NS - 1 units later
     }
     asm volatile("cp.async.wait_group 0;" ::: "memory");
 }
 
-// The reader by name, one per rank (profiles and tests tell the paths apart by it)
-template <int NS, typename T>
+// The reader by name, one per rank (profiles and tests tell the paths apart by it, and the element type by the last
+// template argument)
+template <int NS, bool XFORM, typename T>
 __global__ void __launch_bounds__(256)
 patch_gather_nhwc_host(const T *__restrict__ fmap, const int32_t *__restrict__ randx,
                        const int32_t *__restrict__ randy, float *__restrict__ X, int64_t ldx, int64_t units,
-                       HostGeom g, int relu) {
-    host_reader_body<NS, false>(fmap, randx, randy, X, ldx, units, g, relu);
+                       HostGeom g, int relu, cp_xform xf) {
+    host_reader_body<NS, false, XFORM>(fmap, randx, randy, X, ldx, units, g, relu, xf);
 }
-template <int NS, typename T>
+template <int NS, bool XFORM, typename T>
 __global__ void __launch_bounds__(256)
 patch_gather_ndhwc_host(const T *__restrict__ fmap, const int32_t *__restrict__ randx,
                         const int32_t *__restrict__ randy, float *__restrict__ X, int64_t ldx, int64_t units,
-                        HostGeom g, int relu) {
-    host_reader_body<NS, true>(fmap, randx, randy, X, ldx, units, g, relu);
+                        HostGeom g, int relu, cp_xform xf) {
+    host_reader_body<NS, true, XFORM>(fmap, randx, randy, X, ldx, units, g, relu, xf);
 }
 
 }  // namespace
@@ -162,13 +167,13 @@ static bool host_geom(HostGeom &g, const void *fmap, int esize, int B, int P, in
     return true;
 }
 
-template <int NS, typename T>
+template <int NS, bool XFORM, typename T>
 static void launch_host(const T *fmap, const HostGeom &g, int64_t rows, const int32_t *randx, const int32_t *randy,
-                        int relu, float *X_out, int64_t ldx, int ncta, cudaStream_t stream) {
+                        int relu, const cp_xform &xf, float *X_out, int64_t ldx, int ncta, cudaStream_t stream) {
     const int64_t units = rows * g.nchunk;
     const unsigned grid = (unsigned)(units < ncta ? units : ncta);
-    auto kern = g.randt ? patch_gather_ndhwc_host<NS, T> : patch_gather_nhwc_host<NS, T>;
-    kern<<<grid, 256, (size_t)NS * g.stage, stream>>>(fmap, randx, randy, X_out, ldx, units, g, relu);
+    auto kern = g.randt ? patch_gather_ndhwc_host<NS, XFORM, T> : patch_gather_nhwc_host<NS, XFORM, T>;
+    kern<<<grid, 256, (size_t)NS * g.stage, stream>>>(fmap, randx, randy, X_out, ldx, units, g, relu, xf);
 }
 
 // Grid and pipeline depth of the reader (profiles/host_nhwc_ctas.cu; H100 80GB HBM3 SXM, 700 W; DESIGN.md section 3).
@@ -185,8 +190,9 @@ int cp_patch_gather_host(const cp_patch_args &a) {
                "%s: kernel_size %dx%dx%d too large for the channels-last host reader", a.name, a.g.kt, a.g.kh, a.g.kw);
     cp_with_fmap_type(a.dtype, [&](auto z) {
         using T = decltype(z);
-        launch_host<CP_HOST_NHWC_STAGES>((const T *)a.fmap, g, a.rows(), a.randx, a.randy, a.relu, a.X, a.ldx,
-                                         CP_HOST_NHWC_GATHER_CTAS, a.stream);
+        auto launch = a.fused ? launch_host<CP_HOST_NHWC_STAGES, true, T> : launch_host<CP_HOST_NHWC_STAGES, false, T>;
+        launch((const T *)a.fmap, g, a.rows(), a.randx, a.randy, a.relu, a.xf, a.X, a.ldx, CP_HOST_NHWC_GATHER_CTAS,
+               a.stream);
     });
     CP_CHECK_LAUNCH();
     return CP_OK;

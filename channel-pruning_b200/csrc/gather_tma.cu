@@ -47,6 +47,15 @@ struct GtParams {
     const int32_t *randt;
     int stride_t, pad_t, ngrp;
 };
+// The parameters of the XFORM kernels: + the window and the map extents (which taps lie in the map), and the input
+// transform
+struct GtXParams : GtParams {
+    cp_window g;
+    int D, H, W;
+    cp_xform xf;
+};
+template <bool XFORM>
+using GtArgs = std::conditional_t<XFORM, GtXParams, GtParams>;
 
 __device__ __forceinline__ uint32_t g_smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void g_mbar_init(uint32_t bar, uint32_t count) {
@@ -89,9 +98,12 @@ __device__ __forceinline__ void g_bulk_store(void *gdst, uint32_t ssrc, uint32_t
 }
 __device__ __forceinline__ void g_cons_barrier() { asm volatile("bar.sync 1, %0;" ::"n"(GT_CONS) : "memory"); }
 
-// ND: 4 (NHWC map, whole rows) or 5 (NDHWC map, units of one channel box)
-template <typename T, int K2, int ND>
-__device__ __forceinline__ void gt_body(const CUtensorMap &map, const GtParams &P) {
+// ND: 4 (NHWC map, whole rows) or 5 (NDHWC map, units of one channel box).  XFORM: the input transform P.xf
+// (cp_patch_gather_act).  The copy engine's zero fill is then not enough -- the transform of a zero is not zero once
+// there is a shift -- so the producer hands each stage's window origin and channel offset to the consumers, which
+// find the row's in-map taps (cp_window_tap; a bit mask for the first 32) and write +0 for the others.
+template <typename T, int K2, int ND, bool XFORM>
+__device__ __forceinline__ void gt_body(const CUtensorMap &map, const GtArgs<XFORM> &P) {
     extern __shared__ __align__(128) unsigned char gsm_raw[];
     const int k2 = K2 > 0 ? K2 : P.k2, K = P.c * k2;
     const uint32_t stage_bytes = (uint32_t)K * (uint32_t)sizeof(T), row_bytes = (uint32_t)K * 4u;
@@ -100,6 +112,8 @@ __device__ __forceinline__ void gt_body(const CUtensorMap &map, const GtParams &
     T *in = reinterpret_cast<T *>(base);
     float *out = reinterpret_cast<float *>(in + (size_t)P.nstage * P.stage_f);
     uint64_t *bars = reinterpret_cast<uint64_t *>(out + (size_t)GT_OUT * P.out_f);  // full[nstage], empty[nstage]
+    // XFORM: (t0, y0, x0, channel offset) of the unit in each stage, within the 256 bytes gt_plan adds
+    int *origin = reinterpret_cast<int *>(bars + 2 * P.nstage);
     const int tid = threadIdx.x;
     const uint32_t bar0 = g_smem_u32(bars);
     auto full = [&](int s) { return bar0 + 8u * (uint32_t)s; };
@@ -149,6 +163,10 @@ __device__ __forceinline__ void gt_body(const CUtensorMap &map, const GtParams &
                     const int s = it % P.nstage;
                     const uint32_t ph = (uint32_t)((it / P.nstage) & 1);
                     if (it >= P.nstage) g_mbar_wait(empty(s), ph ^ 1);  // the consumers have released the stage
+                    if constexpr (XFORM) {  // published by the arrive below (release), read after the wait (acquire)
+                        int *o = origin + 4 * s;
+                        o[0] = ts, o[1] = ys, o[2] = xs, o[3] = cs;
+                    }
                     g_mbar_expect_tx(full(s), stage_bytes);
                     const uint32_t dst = g_smem_u32(in + (size_t)s * P.stage_f);
                     for (int b = 0; b < P.nbox; ++b) {
@@ -174,11 +192,32 @@ __device__ __forceinline__ void gt_body(const CUtensorMap &map, const GtParams &
         g_cons_barrier();  // out[o] is no longer being read by the store of row it - GT_OUT
         const T *src = in + (size_t)s * P.stage_f;
         float *dst = out + (size_t)o * P.out_f;
+        int t0 = 0, y0 = 0, x0 = 0, cs = 0;
+        uint32_t inmap = 0;  // bit p: tap p < 32 lies in the map
+        if constexpr (XFORM) {
+            const int *og = origin + 4 * s;
+            t0 = og[0], y0 = og[1], x0 = og[2], cs = og[3];
+            const int nb = k2 < 32 ? k2 : 32;
+            for (int p = 0; p < nb; ++p) {
+                int tt, yy, xx;
+                inmap |= (uint32_t)cp_window_tap<ND == 5>(P.g, p, t0, y0, x0, P.D, P.H, P.W, tt, yy, xx) << p;
+            }
+        }
+        // XFORM: the value of tap p of channel a (within the unit) as it is stored (Q: P, a GtXParams)
+        auto xput = [&](const auto &Q, float v, int p, int a) {
+            int tt, yy, xx;
+            const bool in = p < 32 ? (inmap >> p) & 1u
+                                   : cp_window_tap<ND == 5>(Q.g, p, t0, y0, x0, Q.D, Q.H, Q.W, tt, yy, xx);
+            return in ? cp_xform_apply(Q.xf, v, cs + a) : 0.f;
+        };
         for (int a = tid; a < P.c; a += GT_CONS) {
             const int b = a / P.cbox, al = a - b * P.cbox;
             const T *sp = src + (size_t)b * P.box_f + al;
             float *dp = dst + (size_t)a * k2;
-            if (K2 > 0) {
+            if constexpr (XFORM) {
+                // one tap at a time: the transform's division and expf leave no registers for a batch of loads
+                for (int p = 0; p < k2; ++p) dp[p] = xput(P, cp_widen(sp[(size_t)p * P.cbox]), p, a);
+            } else if (K2 > 0) {
                 // loads of a slab batched ahead of its stores; a 3 x 3 x 3 window goes by 3 x 3 slabs (registers)
                 constexpr int KS = K2 > 9 && K2 % 9 == 0 ? 9 : (K2 > 0 ? K2 : 1);
 #pragma unroll
@@ -215,15 +254,15 @@ __device__ __forceinline__ void gt_body(const CUtensorMap &map, const GtParams &
 
 // The kernel by name, one per rank of the tensor map (profiles and tests tell the paths apart by it); T: map element
 // type; K2: taps known at compile time (gt_launch) or 0
-template <typename T, int K2>
+template <typename T, int K2, bool XFORM = false>
 __global__ void __launch_bounds__(GT_THREADS)
-patch_gather_nhwc_tma(const __grid_constant__ CUtensorMap map, const GtParams P) {
-    gt_body<T, K2, 4>(map, P);
+patch_gather_nhwc_tma(const __grid_constant__ CUtensorMap map, const GtArgs<XFORM> P) {
+    gt_body<T, K2, 4, XFORM>(map, P);
 }
-template <typename T, int K2>
+template <typename T, int K2, bool XFORM = false>
 __global__ void __launch_bounds__(GT_THREADS)
-patch_gather_ndhwc_tma(const __grid_constant__ CUtensorMap map, const GtParams P) {
-    gt_body<T, K2, 5>(map, P);
+patch_gather_ndhwc_tma(const __grid_constant__ CUtensorMap map, const GtArgs<XFORM> P) {
+    gt_body<T, K2, 5, XFORM>(map, P);
 }
 
 inline size_t gt_round128(size_t b) { return (b + 127) & ~(size_t)127; }
@@ -242,18 +281,20 @@ typedef CUresult (*encode_fn_t)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, 
 
 }  // namespace
 
-typedef void (*gt_kernel_t)(const CUtensorMap, const GtParams);
+template <bool XFORM>
+using gt_kernel_t = void (*)(const CUtensorMap, const GtArgs<XFORM>);
 
-template <int ND, typename T, int K2>
-static gt_kernel_t gt_kernel() {
+template <int ND, typename T, int K2, bool XFORM>
+static gt_kernel_t<XFORM> gt_kernel() {
     if constexpr (ND == 4)
-        return patch_gather_nhwc_tma<T, K2>;
+        return patch_gather_nhwc_tma<T, K2, XFORM>;
     else
-        return patch_gather_ndhwc_tma<T, K2>;
+        return patch_gather_ndhwc_tma<T, K2, XFORM>;
 }
 
-static int gt_run(cp_handle_t h, gt_kernel_t kern, cp_per_device_flag &configured, const CUtensorMap &map,
-                  const GtParams &Pm, size_t smem, int per_sm, cudaStream_t stream) {
+template <bool XFORM>
+static int gt_run(cp_handle_t h, gt_kernel_t<XFORM> kern, cp_per_device_flag &configured, const CUtensorMap &map,
+                  const GtArgs<XFORM> &Pm, size_t smem, int per_sm, cudaStream_t stream) {
     if (bool *done = configured.slot(); !*done) {
         CP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
         *done = true;
@@ -267,16 +308,16 @@ static int gt_run(cp_handle_t h, gt_kernel_t kern, cp_per_device_flag &configure
 
 // One instantiation per (rank, element type, taps): 1 x 1 and 3 x 3 windows of either rank, 5 x 5 of 2-D maps and
 // 3 x 3 x 3 of 3-D maps at compile time (a dilated window takes the instantiation of its tap count), the rest K2 = 0
-template <int ND, typename T>
-static int gt_launch(cp_handle_t h, const CUtensorMap &map, const GtParams &Pm, size_t smem, int per_sm,
+template <int ND, typename T, bool XFORM>
+static int gt_launch(cp_handle_t h, const CUtensorMap &map, const GtArgs<XFORM> &Pm, size_t smem, int per_sm,
                      cudaStream_t stream) {
     constexpr int KBIG = ND == 4 ? 25 : 27;
     const int k2 = Pm.k2;
-    auto kern = k2 == 9 ? gt_kernel<ND, T, 9>() : k2 == 1 ? gt_kernel<ND, T, 1>()
-              : k2 == KBIG ? gt_kernel<ND, T, KBIG>() : gt_kernel<ND, T, 0>();
-    static cp_per_device_flag configured[4];  // one set per (rank, element type): one per instantiation of gt_launch
+    auto kern = k2 == 9 ? gt_kernel<ND, T, 9, XFORM>() : k2 == 1 ? gt_kernel<ND, T, 1, XFORM>()
+              : k2 == KBIG ? gt_kernel<ND, T, KBIG, XFORM>() : gt_kernel<ND, T, 0, XFORM>();
+    static cp_per_device_flag configured[4];  // one set per (rank, element type, XFORM): per instantiation of gt_launch
     const int which = k2 == 9 ? 0 : k2 == 1 ? 1 : k2 == KBIG ? 2 : 3;
-    return gt_run(h, kern, configured[which], map, Pm, smem, per_sm, stream);
+    return gt_run<XFORM>(h, kern, configured[which], map, Pm, smem, per_sm, stream);
 }
 
 // CTAs per SM and input stages for a window stage of `row` bytes and output rows of `out_b` bytes: as many CTAs as fit
@@ -358,6 +399,7 @@ static bool gt_plan(GtPlan &pl, int esize, int c, const cp_window &g, bool depth
     // for fp32 the stage is never smaller than the output
     if (2 * pl.row + GT_OUT * (pl.row > pl.out_b ? pl.row : pl.out_b) + 1024 > 200 * 1024) return false;
     gt_ring(pl.row, pl.out_b, pl.per_sm, pl.nstage);
+    // + 256: the 128-byte alignment of the base, and the XFORM kernels' stage origins (16 bytes per stage, nstage <= 6)
     pl.smem = (size_t)pl.nstage * pl.row + GT_OUT * pl.out_b + 2 * pl.nstage * 8 + 256;
     return true;
 }
@@ -405,7 +447,7 @@ int cp_patch_gather_tma(cp_handle_t h, const cp_patch_args &a) {
     CUtensorMap map;
     if (int rc = gt_encode(h, map, a, pl)) return rc;
     const cp_window &g = a.g;
-    GtParams Pm{};
+    GtXParams Pm{};
     Pm.randx = a.randx; Pm.randy = a.randy; Pm.randt = a.randt; Pm.X = a.X; Pm.ldx = a.ldx;
     Pm.ngrp = pl.ngrp;
     Pm.rows = a.rows() * pl.ngrp;  // work units
@@ -414,9 +456,13 @@ int cp_patch_gather_tma(cp_handle_t h, const cp_patch_args &a) {
     Pm.stride_t = g.stride_t; Pm.stride_h = g.stride_h; Pm.stride_w = g.stride_w;
     Pm.cbox = pl.cbox; Pm.nbox = pl.nbox; Pm.nstage = pl.nstage;
     Pm.box_f = (int)(pl.box_b / esize); Pm.stage_f = (int)(pl.row / esize); Pm.out_f = (int)(pl.out_b / 4);
+    Pm.g = g; Pm.D = a.D; Pm.H = a.H; Pm.W = a.W; Pm.xf = a.xf;
     return cp_with_fmap_type(a.dtype, [&](auto z) {
         using T = decltype(z);
-        return pl.rank == 5 ? gt_launch<5, T>(h, map, Pm, pl.smem, pl.per_sm, a.stream)
-                            : gt_launch<4, T>(h, map, Pm, pl.smem, pl.per_sm, a.stream);
+        if (a.fused)
+            return pl.rank == 5 ? gt_launch<5, T, true>(h, map, Pm, pl.smem, pl.per_sm, a.stream)
+                                : gt_launch<4, T, true>(h, map, Pm, pl.smem, pl.per_sm, a.stream);
+        return pl.rank == 5 ? gt_launch<5, T, false>(h, map, Pm, pl.smem, pl.per_sm, a.stream)
+                            : gt_launch<4, T, false>(h, map, Pm, pl.smem, pl.per_sm, a.stream);
     });
 }

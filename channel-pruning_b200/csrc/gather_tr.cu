@@ -18,7 +18,8 @@
 //       to (c, taps) order
 // A map in pinned host memory is read in place by the same kernel with a small persistent grid (PCIe-bound: more CTAs
 // only block SMs that other layers need).  The values are widened exactly and the ReLU is applied with the expression
-// of the conv gathers (gather.cu), so -0, inf and NaN come out as the conv gathers give them.
+// of the conv gathers (gather.cu), so -0, inf and NaN come out as the conv gathers give them; the XFORM = true kernels
+// apply cp_patch_gather_act's input transform to the valid taps instead, and leave the invalid ones +0.
 #include "common.cuh"
 #include "fmap_types.cuh"
 
@@ -85,11 +86,12 @@ __device__ __forceinline__ void tr_valid_tap(const tr_row &q, const cp_window &g
 
 // Channels first: grid-stride over the rows (grid = rows in HBM, a small persistent grid for a pinned host map).
 // Shared: k pixel offsets, -1 for an invalid tap.
-template <bool DEPTH, typename T>
+template <bool DEPTH, bool XFORM, typename T>
 __device__ __forceinline__ void tr_cfirst_body(const T *__restrict__ fmap, const int32_t *__restrict__ randt,
                                                const int32_t *__restrict__ randx, const int32_t *__restrict__ randy,
                                                float *__restrict__ X, int64_t ldx, int64_t rows, int B, int c, int D,
-                                               int H, int W, int P, const cp_window &g, int relu) {
+                                               int H, int W, int P, const cp_window &g, int relu,
+                                               const cp_xform &xf) {
     extern __shared__ int64_t tap_pix[];
     const int k = (DEPTH ? g.kt : 1) * g.kh * g.kw;
     const int K = c * k;
@@ -114,8 +116,11 @@ __device__ __forceinline__ void tr_cfirst_body(const T *__restrict__ fmap, const
             const int a = col / k;
             const int64_t pix = tap_pix[col - a * k];
             float v = 0.f;
-            if (pix >= 0) v = cp_widen(__ldg(src + a * plane + pix));
-            if (relu) v = fmaxf(v, 0.f);
+            if (pix >= 0) {
+                v = cp_widen(__ldg(src + a * plane + pix));
+                if (XFORM) v = cp_xform_apply(xf, v, a);
+            }
+            if (!XFORM && relu) v = fmaxf(v, 0.f);
             dst[col] = v;
         }
         __syncthreads();  // the table is rebuilt for the next row
@@ -125,26 +130,26 @@ __device__ __forceinline__ void tr_cfirst_body(const T *__restrict__ fmap, const
 #define CP_TR_CFIRST_PARAMS                                                                                           \
     const T *__restrict__ fmap, const int32_t *__restrict__ randt, const int32_t *__restrict__ randx,                  \
         const int32_t *__restrict__ randy, float *__restrict__ X, int64_t ldx, int64_t rows, int B, int c, int D, int H, \
-        int W, int P, cp_window g, int relu
-template <typename T>
+        int W, int P, cp_window g, int relu, cp_xform xf
+template <typename T, bool XFORM = false>
 __global__ void __launch_bounds__(256) patch_gather_tr_nchw(CP_TR_CFIRST_PARAMS) {
-    tr_cfirst_body<false>(fmap, nullptr, randx, randy, X, ldx, rows, B, c, 1, H, W, P, g, relu);
+    tr_cfirst_body<false, XFORM>(fmap, nullptr, randx, randy, X, ldx, rows, B, c, 1, H, W, P, g, relu, xf);
 }
-template <typename T>
+template <typename T, bool XFORM = false>
 __global__ void __launch_bounds__(256) patch_gather_tr_ncdhw(CP_TR_CFIRST_PARAMS) {
-    tr_cfirst_body<true>(fmap, randt, randx, randy, X, ldx, rows, B, c, D, H, W, P, g, relu);
+    tr_cfirst_body<true, XFORM>(fmap, randt, randx, randy, X, ldx, rows, B, c, D, H, W, P, g, relu, xf);
 }
 
 // Channels last: grid-stride over the units (output row, channel tile of ct_tile channels).  Shared: k slots (index of
 // tap p among the row's valid taps, -1 when invalid), then the tile [nvmax][ct_tile + 1] of the valid taps' channels
 // (widened, ReLU applied; ct_tile + 1: the transposed read is conflict-free).  VE > 1: 16-byte loads of VE elements
 // (the launcher's rules: c and ct_tile multiples of VE, 16-byte aligned map).
-template <bool DEPTH, int VE, typename T>
+template <bool DEPTH, int VE, bool XFORM, typename T>
 __device__ __forceinline__ void tr_clast_body(const T *__restrict__ fmap, const int32_t *__restrict__ randt,
                                               const int32_t *__restrict__ randx, const int32_t *__restrict__ randy,
                                               float *__restrict__ X, int64_t ldx, int64_t units, int ntile, int B,
                                               int c, int D, int H, int W, int P, const cp_window &g, int ct_tile,
-                                              int tile_off, int relu) {
+                                              int tile_off, int relu, const cp_xform &xf) {
     extern __shared__ __align__(16) unsigned char tr_smem[];
     int *slot = reinterpret_cast<int *>(tr_smem);
     float *tile = reinterpret_cast<float *>(tr_smem + tile_off);
@@ -177,12 +182,14 @@ __device__ __forceinline__ void tr_clast_body(const T *__restrict__ fmap, const 
 #pragma unroll
                 for (int m = 0; m < VE; ++m) {
                     float x = cp_widen(w.e[m]);
-                    if (relu) x = fmaxf(x, 0.f);
+                    if (XFORM) x = cp_xform_apply(xf, x, a0 + jv * VE + m);
+                    else if (relu) x = fmaxf(x, 0.f);
                     t[m] = x;
                 }
             } else {
                 float x = cp_widen(__ldg(src + pix * c + jv));
-                if (relu) x = fmaxf(x, 0.f);
+                if (XFORM) x = cp_xform_apply(xf, x, a0 + jv);
+                else if (relu) x = fmaxf(x, 0.f);
                 t[0] = x;
             }
         }
@@ -191,7 +198,7 @@ __device__ __forceinline__ void tr_clast_body(const T *__restrict__ fmap, const 
         for (int e = threadIdx.x; e < k * ct; e += blockDim.x) {
             const int a = e / k;
             const int s = slot[e - a * k];
-            dst[e] = s >= 0 ? tile[s * ld + a] : 0.f;  // the ReLU of a zero tap is +0
+            dst[e] = s >= 0 ? tile[s * ld + a] : 0.f;  // the ReLU of a zero tap is +0; the transform skips it
         }
         __syncthreads();  // slots and tile are rebuilt for the next unit
     }
@@ -200,16 +207,16 @@ __device__ __forceinline__ void tr_clast_body(const T *__restrict__ fmap, const 
 #define CP_TR_CLAST_PARAMS                                                                                            \
     const T *__restrict__ fmap, const int32_t *__restrict__ randt, const int32_t *__restrict__ randx,                  \
         const int32_t *__restrict__ randy, float *__restrict__ X, int64_t ldx, int64_t units, int ntile, int B, int c,   \
-        int D, int H, int W, int P, cp_window g, int ct_tile, int tile_off, int relu
-template <int VE, typename T>
+        int D, int H, int W, int P, cp_window g, int ct_tile, int tile_off, int relu, cp_xform xf
+template <int VE, typename T, bool XFORM = false>
 __global__ void __launch_bounds__(256) patch_gather_tr_nhwc(CP_TR_CLAST_PARAMS) {
-    tr_clast_body<false, VE>(fmap, nullptr, randx, randy, X, ldx, units, ntile, B, c, 1, H, W, P, g, ct_tile, tile_off,
-                             relu);
+    tr_clast_body<false, VE, XFORM>(fmap, nullptr, randx, randy, X, ldx, units, ntile, B, c, 1, H, W, P, g, ct_tile,
+                                    tile_off, relu, xf);
 }
-template <int VE, typename T>
+template <int VE, typename T, bool XFORM = false>
 __global__ void __launch_bounds__(256) patch_gather_tr_ndhwc(CP_TR_CLAST_PARAMS) {
-    tr_clast_body<true, VE>(fmap, randt, randx, randy, X, ldx, units, ntile, B, c, D, H, W, P, g, ct_tile, tile_off,
-                            relu);
+    tr_clast_body<true, VE, XFORM>(fmap, randt, randx, randy, X, ldx, units, ntile, B, c, D, H, W, P, g, ct_tile,
+                                   tile_off, relu, xf);
 }
 
 // Grids of the in-place readers of pinned host maps: those of the conv gathers' channels-first and channels-last
@@ -229,7 +236,7 @@ int tr_max_taps(int k, int s, int d) {
     return (k + period - 1) / period;
 }
 
-template <typename T>
+template <typename T, bool XFORM>
 void launch_tr(const cp_patch_args &a, bool host_src) {
     const cp_window &g = a.g;
     const T *fmap = (const T *)a.fmap;
@@ -239,9 +246,9 @@ void launch_tr(const cp_patch_args &a, bool host_src) {
     const int64_t grid_max = 0x7fffffff;
     if (a.layout == CP_LAYOUT_NCHW) {
         const int64_t grid = host_src ? std::min(rows, TR_HOST_CFIRST_CTAS) : rows;
-        auto kern = depth ? patch_gather_tr_ncdhw<T> : patch_gather_tr_nchw<T>;
+        auto kern = depth ? patch_gather_tr_ncdhw<T, XFORM> : patch_gather_tr_nchw<T, XFORM>;
         kern<<<(unsigned)grid, 256, (size_t)k * sizeof(int64_t), a.stream>>>(
-            fmap, a.randt, a.randx, a.randy, a.X, a.ldx, rows, a.B, a.c, a.D, a.H, a.W, a.P, g, a.relu);
+            fmap, a.randt, a.randx, a.randy, a.X, a.ldx, rows, a.B, a.c, a.D, a.H, a.W, a.P, g, a.relu, a.xf);
         return;
     }
     const int nvmax = tr_max_taps(g.kt, g.stride_t, g.dil_t) * tr_max_taps(g.kh, g.stride_h, g.dil_h) *
@@ -259,10 +266,10 @@ void launch_tr(const cp_patch_args &a, bool host_src) {
     const int64_t units = rows * ntile;
     const int64_t grid = std::min(host_src ? TR_HOST_CLAST_CTAS : grid_max, units);
     const size_t smem = (size_t)tile_off + (size_t)nvmax * (ct_tile + 1) * sizeof(float);
-    auto kern = vec ? (depth ? patch_gather_tr_ndhwc<VE, T> : patch_gather_tr_nhwc<VE, T>)
-                    : (depth ? patch_gather_tr_ndhwc<1, T> : patch_gather_tr_nhwc<1, T>);
+    auto kern = vec ? (depth ? patch_gather_tr_ndhwc<VE, T, XFORM> : patch_gather_tr_nhwc<VE, T, XFORM>)
+                    : (depth ? patch_gather_tr_ndhwc<1, T, XFORM> : patch_gather_tr_nhwc<1, T, XFORM>);
     kern<<<(unsigned)grid, 256, smem, a.stream>>>(fmap, a.randt, a.randx, a.randy, a.X, a.ldx, units, ntile, a.B, a.c,
-                                                  a.D, a.H, a.W, a.P, g, ct_tile, tile_off, a.relu);
+                                                  a.D, a.H, a.W, a.P, g, ct_tile, tile_off, a.relu, a.xf);
 }
 
 }  // namespace
@@ -270,7 +277,12 @@ void launch_tr(const cp_patch_args &a, bool host_src) {
 // gather.cu's entries call this once the arguments passed its checks (rows > 0); host_src: the map lies in pinned
 // host memory
 int cp_patch_gather_tr(const cp_patch_args &a, bool host_src) {
-    cp_with_fmap_type(a.dtype, [&](auto z) { launch_tr<decltype(z)>(a, host_src); });
+    cp_with_fmap_type(a.dtype, [&](auto z) {
+        if (a.fused)
+            launch_tr<decltype(z), true>(a, host_src);
+        else
+            launch_tr<decltype(z), false>(a, host_src);
+    });
     CP_CHECK_LAUNCH();
     return CP_OK;
 }

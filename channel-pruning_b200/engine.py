@@ -60,6 +60,40 @@ def fmap_dtype_code(dtype):
     return code
 
 
+# the activations of a consumer's input transform: name -> CP_ACT_* of include/cpb200.h
+ACTS = {"identity": 0, "relu": 1, "relu6": 2, "leaky_relu": 3, "hardswish": 4, "silu": 5}
+LEAKY_SLOPE = 0.01  # torch.nn.LeakyReLU's default negative_slope
+
+
+def check_act(act, act_param):
+    """ValueError for an activation not in ACTS, or a slope given to an activation other than leaky_relu."""
+    if act not in ACTS:
+        raise ValueError("unknown activation %r (one of %s)" % (act, ", ".join(ACTS)))
+    if act_param is not None and act != "leaky_relu":
+        raise ValueError("act_param (the negative slope) is an argument of leaky_relu, not of %r" % act)
+
+
+def input_transform(relu, act, act_param, in_scale, in_shift, c, device):
+    """The input transform a gather was asked for: None for the relu flag's gathers (relu True / None, or act 'relu',
+    without an affine; relu False or act 'identity' likewise), else (CP_ACT code, slope, scale, shift).  relu and act
+    exclude each other; scale and shift are contiguous fp32 tensors of c values on device, or None."""
+    if relu is not None and act is not None:
+        raise ValueError("pass relu or act, not both")
+    if act is None:
+        if act_param is not None:
+            raise ValueError("act_param without act")
+        act = "identity" if relu is False else "relu"
+    check_act(act, act_param)
+    for t in (in_scale, in_shift):
+        if t is not None:
+            assert t.dtype == torch.float32 and t.is_contiguous() and t.numel() == c, "scale / shift: %d fp32" % c
+            assert t.is_cuda and t.device == device, "scale / shift must live on %s" % device
+    if act in ("relu", "identity") and in_scale is None and in_shift is None:
+        return None
+    slope = float(LEAKY_SLOPE if act_param is None else act_param) if act == "leaky_relu" else 0.0
+    return ACTS[act], slope, in_scale, in_shift
+
+
 def _gather_map(fmap, B, layout, d3):
     """(dtype code, layout code, nbatch, dims) of a gather's map (nbatch*B images): dims is (c, H, W) of a 2-D map and
     (c, D, H, W) of a 3-D one (d3), c the channels whichever the layout.  TypeError for a dtype the gathers do not read,
@@ -258,8 +292,8 @@ class Engine:
         return torch.empty(*shape, dtype=dtype, device=self.device)
 
     # ------------------------------------------------------------------ kernels
-    def patch_gather(self, fmap, randx, randy, B, P, k, pad, stride, relu=True, layout="nchw", out=None, dilation=1,
-                     transposed=False):
+    def patch_gather(self, fmap, randx, randy, B, P, k, pad, stride, relu=None, layout="nchw", out=None, dilation=1,
+                     transposed=False, act=None, act_param=None, in_scale=None, in_shift=None):
         """fmap: (nbatch*B, c, H, W) [nchw] or (nbatch*B, H, W, c) [nhwc], float32 / bfloat16 / float16, on device
         or in pinned host memory (read in place over PCIe); randx/randy: (nbatch, P) int32 on device.  Returns X (nbatch*P*B, c*kh*kw)
         fp32 -- 16-bit maps are widened exactly, so X equals the X of fmap.float().
@@ -268,9 +302,17 @@ class Engine:
         All ints with dilation 1 is the reference's window, which must be odd (an even square kernel is (k, k)).
         transposed: the window of torch.nn.ConvTranspose2d (k, pad = padding, stride, dilation as it takes them; fmap
         its input map, the points in its output map; cp_patch_gather_conv_transpose).  Then X @
-        weight.transpose(0, 1).reshape(n, -1).T is the layer's output at the points, minus its bias."""
+        weight.transpose(0, 1).reshape(n, -1).T is the layer's output at the points, minus its bias.
+        relu: True (the default) or False, the ReLU of the reference's VGG maps.  act, act_param, in_scale, in_shift
+        instead: the consumer's input transform of a Conv-BN-activation network whose map is the producer's raw conv
+        output (input_transform; cp_patch_gather_act).  relu and act exclude each other."""
         geo = _gather_map(fmap, B, layout, False)
         (kh, kw), (ph, pw), (sh, sw), (dh, dw) = (conv_pair(v) for v in (k, pad, stride, dilation))
+        xf = input_transform(relu, act, act_param, in_scale, in_shift, geo[3][0], self.device)
+        if xf is not None:
+            window = (1, kh, kw, 0, ph, pw, 1, sh, sw, 1, dh, dw)
+            return self._patch_gather_act(geo, fmap, (None, randx, randy), B, P, kh * kw, window, transposed, xf, out)
+        relu = relu is None or relu if act is None else act == "relu"
         if transposed:
             fn, window = self.lib.cp_patch_gather_conv_transpose, (kh, kw, ph, pw, sh, sw, dh, dw)
         elif all(isinstance(v, (int, np.integer)) for v in (k, pad, stride, dilation)) and dilation == 1:
@@ -284,19 +326,25 @@ class Engine:
         geo = _gather_map(fmap, B, layout, False)
         return self._point_gather(self.lib.cp_point_gather_typed, geo, fmap, (randx, randy), B, P, out)
 
-    def patch_gather3d(self, fmap, randt, randx, randy, B, P, k, pad, stride, relu=True, layout="ncdhw", out=None,
-                       dilation=1, transposed=False):
+    def patch_gather3d(self, fmap, randt, randx, randy, B, P, k, pad, stride, relu=None, layout="ncdhw", out=None,
+                       dilation=1, transposed=False, act=None, act_param=None, in_scale=None, in_shift=None):
         """fmap: (nbatch*B, c, D, H, W) [ncdhw] or (nbatch*B, D, H, W, c) [ndhwc, channels_last_3d], float32 /
         bfloat16 / float16, on device or in pinned host memory (read in place); randt/randx/randy: (nbatch, P) int32 on
         device, the sampled output points (t, x, y).  Returns X (nbatch*P*B, c*kt*kh*kw) fp32, 16-bit maps widened
         exactly.  k, pad, stride, dilation: an int or a (t, h, w) triple, with the meaning of torch.nn.Conv3d's
         arguments (pad: the front / top / left padding).  Columns are in Conv3d.weight.reshape(n, -1)'s order.
-        transposed: the window of torch.nn.ConvTranspose3d, as for patch_gather (cp_patch_gather_conv_transpose3d)."""
+        transposed: the window of torch.nn.ConvTranspose3d, as for patch_gather (cp_patch_gather_conv_transpose3d).
+        relu, act, act_param, in_scale, in_shift: as for patch_gather."""
         geo = _gather_map(fmap, B, layout, True)
         (kt, kh, kw), (pt, ph, pw), (st, sh, sw), (dt, dh, dw) = (conv_triple(v) for v in (k, pad, stride, dilation))
+        window = (kt, kh, kw, pt, ph, pw, st, sh, sw, dt, dh, dw)
+        xf = input_transform(relu, act, act_param, in_scale, in_shift, geo[3][0], self.device)
+        if xf is not None:
+            return self._patch_gather_act(geo, fmap, (randt, randx, randy), B, P, kt * kh * kw, window, transposed, xf,
+                                          out)
         fn = self.lib.cp_patch_gather_conv_transpose3d if transposed else self.lib.cp_patch_gather_conv3d
-        return self._patch_gather(fn, geo, fmap, (randt, randx, randy), B, P,
-                                  kt * kh * kw, (kt, kh, kw, pt, ph, pw, st, sh, sw, dt, dh, dw), relu, out)
+        relu = relu is None or relu if act is None else act == "relu"
+        return self._patch_gather(fn, geo, fmap, (randt, randx, randy), B, P, kt * kh * kw, window, relu, out)
 
     def point_gather3d(self, fmap, randt, randx, randy, B, P, layout="ncdhw", out=None):
         """Y (nbatch*P*B, n) fp32 at the sampled points (t, x, y) of a Conv3d output map (nbatch*B, n, To, Ho, Wo)
@@ -318,6 +366,27 @@ class Engine:
         self._call(fn(self.h, self._p(fmap, "const void*"), dt, nbatch, B, *dims, lay,
                       *[self._p(r, "const int32_t*") for r in points], P, *window, int(bool(relu)),
                       self._p(out, "float*"), out.stride(0), self._s()))
+        return out
+
+    def _patch_gather_act(self, geo, fmap, points, B, P, taps, window, transposed, xf, out):
+        """patch_gather and patch_gather3d through cp_patch_gather_act: points (randt or None, randx, randy), window
+        the 12 values kt ... dil_w, xf what input_transform returned."""
+        dt, lay, nbatch, dims = geo
+        if len(dims) == 3:
+            dims = (dims[0], 1) + tuple(dims[1:])  # (c, D = 1, H, W)
+        assert fmap.shape[0] % B == 0
+        for r in points[1:] if points[0] is None else points:
+            assert r.dtype == torch.int32 and r.numel() == nbatch * P and r.is_contiguous()
+        rows, K = nbatch * P * B, dims[0] * taps
+        if out is None:
+            out = self.empty(rows, K, dtype=torch.float32)
+        assert out.shape == (rows, K) and out.dtype == torch.float32 and out.stride(1) == 1
+        act, slope, scale, shift = xf
+        self._call(self.lib.cp_patch_gather_act(
+            self.h, self._p(fmap, "const void*"), dt, nbatch, B, *dims, lay,
+            *[self._p(r, "const int32_t*") for r in points], P, *window, int(bool(transposed)), act, slope,
+            self._p(scale, "const float*"), self._p(shift, "const float*"), self._p(out, "float*"), out.stride(0),
+            self._s()))
         return out
 
     def _point_gather(self, fn, geo, fmap, points, B, P, out):

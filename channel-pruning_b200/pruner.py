@@ -167,11 +167,14 @@ def _default_layout(s):
 
 def _patch_gather(eng, s, d, fmap, layout):
     """The gather of layer s from map fmap (layout as the map lies): Engine.patch_gather3d for a Conv3d layer
-    (d carries randt), Engine.patch_gather otherwise."""
+    (d carries randt), Engine.patch_gather otherwise; through the shape's input transform (s.act, s.act_param; the
+    ReLU when the shape has none) and the problem's affine (d['in_scale'], d['in_shift'], when present)."""
+    xf = dict(act=getattr(s, "act", "relu"), act_param=getattr(s, "act_param", None), in_scale=d.get("in_scale"),
+              in_shift=d.get("in_shift"))
     if _is3d(s):
-        return eng.patch_gather3d(fmap, d["randt"], d["randx"], d["randy"], s.B, s.P, relu=True, layout=layout,
+        return eng.patch_gather3d(fmap, d["randt"], d["randx"], d["randy"], s.B, s.P, layout=layout, **xf,
                                   **s.conv_args())
-    return eng.patch_gather(fmap, d["randx"], d["randy"], s.B, s.P, relu=True, layout=layout, **s.conv_args())
+    return eng.patch_gather(fmap, d["randx"], d["randy"], s.B, s.P, layout=layout, **xf, **s.conv_args())
 
 
 def zero_copy_lines(s, esize=4, layout="nchw"):

@@ -17,7 +17,7 @@ from __future__ import annotations
 
 import numpy as np
 
-from .engine import conv_pair, conv_triple
+from .engine import LEAKY_SLOPE, check_act, conv_pair, conv_triple
 
 # (name, c_in, n_out, H=W of the layer's input/output map)  -- temp/vgg.prototxt:53-306
 VGG16 = [
@@ -75,6 +75,12 @@ def _out_size(n, k, pad, stride, dil, output_padding, transposed):
     return out
 
 
+def _set_input(s, act, act_param, bn):
+    """The consumer's input transform of a layer shape: act (engine.ACTS) after, with bn, the producer's BatchNorm."""
+    check_act(act, act_param)
+    s.act, s.act_param, s.bn = act, act_param, bool(bn)
+
+
 def _conv_args(s):
     a = dict(k=s.k, pad=s.pad, stride=s.stride, dilation=s.dilation)
     if s.transposed:
@@ -89,10 +95,14 @@ class LayerShape:
     kh, kw, pad_h, pad_w, stride_h, stride_w, dil_h, dil_w: the per-axis geometry; k2 = kh*kw taps per channel;
     Ho x Wo: the output map (PyTorch's formula), the range of the sampled points.
     transposed: a torch.nn.ConvTranspose2d consumer (k, pad = padding, stride, dilation and output_padding as it takes
-    them; H x W its input map); W2 is then (n, c, kh, kw) = weight.transpose(0, 1), the orientation of every layer."""
+    them; H x W its input map); W2 is then (n, c, kh, kw) = weight.transpose(0, 1), the orientation of every layer.
+    act, act_param, bn: the consumer's input transform (Engine.patch_gather).  The map is the producer's raw conv output
+    and X is act(BN(map)) with bn (the problem's in_scale / in_shift, fold_bn of the producer's BatchNorm), act(map)
+    without; act 'relu' and no bn is the reference's VGG layer."""
 
     def __init__(self, name, c, n, H, k=3, pad=1, stride=1, N=5000, B=10, P=10, rank=None, dilation=1, W=None,
-                 transposed=False, output_padding=0):
+                 transposed=False, output_padding=0, act="relu", act_param=None, bn=False):
+        _set_input(self, act, act_param, bn)
         self.name, self.c, self.n, self.H, self.W = name, c, n, H, H if W is None else W
         self.k, self.pad, self.stride, self.dilation = k, pad, stride, dilation
         self.transposed, self.output_padding = bool(transposed), output_padding
@@ -129,10 +139,12 @@ class LayerShape3d:
     given).  k, pad, stride and dilation are ints or (t, h, w) triples, as torch.nn.Conv3d takes them (groups == 1).
     kt, kh, kw, pad_t, ..., dil_w: the per-axis geometry; k2 = kt*kh*kw taps per channel (what the solver sees: X is
     (N, c*k2)); To x Ho x Wo: the output map (PyTorch's formula), the range of the sampled points (t, x, y).
-    transposed, output_padding: a torch.nn.ConvTranspose3d consumer, as for LayerShape."""
+    transposed, output_padding: a torch.nn.ConvTranspose3d consumer; act, act_param, bn: its input transform; as for
+    LayerShape."""
 
     def __init__(self, name, c, n, D, H, k=3, pad=1, stride=1, N=5000, B=10, P=10, rank=None, dilation=1, W=None,
-                 transposed=False, output_padding=0):
+                 transposed=False, output_padding=0, act="relu", act_param=None, bn=False):
+        _set_input(self, act, act_param, bn)
         self.name, self.c, self.n, self.D, self.H, self.W = name, c, n, D, H, H if W is None else W
         self.k, self.pad, self.stride, self.dilation = k, pad, stride, dilation
         self.transposed, self.output_padding = bool(transposed), output_padding
@@ -218,15 +230,93 @@ def vgg16_layers(N=5000, B=10, P=10):
     return [LayerShape(nm, c, n, H, N=N, B=B, P=P) for nm, c, n, H in VGG16]
 
 
-def resnet50_layers(N=5000, B=10, P=10):
-    return [LayerShape(nm, c, n, H, k=k, pad=pad, stride=st, N=N, B=B, P=P, rank=kept)
+def resnet50_layers(N=5000, B=10, P=10, bn=False):
+    """The 48 bottleneck convolutions of RESNET50.  bn: pruned from the raw conv outputs of a Conv-BN-ReLU network --
+    branch2b and branch2c take ReLU(BN(raw output of the branch before)); branch2a keeps the ReLU of its input, the
+    block's post-add map."""
+    return [LayerShape(nm, c, n, H, k=k, pad=pad, stride=st, N=N, B=B, P=P, rank=kept,
+                       bn=bn and not nm.endswith("branch2a"))
             for nm, c, n, k, H, st, pad, kept in RESNET50]
+
+
+def fold_bn(bn):
+    """(scale, shift) of an eval-mode torch.nn.BatchNorm2d / 3d: scale = weight / sqrt(running_var + eps), shift =
+    bias - running_mean * scale, computed in float64 and rounded once to float32 (contiguous tensors on bn's device).
+    bn itself is left untouched."""
+    import torch
+
+    with torch.no_grad():
+        var, mean = bn.running_var.double(), bn.running_mean.double()
+        w = bn.weight.double() if bn.weight is not None else torch.ones_like(var)
+        b = bn.bias.double() if bn.bias is not None else torch.zeros_like(var)
+        scale = w / torch.sqrt(var + bn.eps)
+        shift = b - mean * scale
+        return scale.float().contiguous(), shift.float().contiguous()
+
+
+def input_transform_numpy(v, act, act_param=None, scale=None, shift=None):
+    """The consumer's input transform (cpb200.h, cp_patch_gather_act) on float32 values v, channels on axis 1:
+    (v * scale) + shift, each rounded in float32 (either left out when None), then act.  Every act but silu is the
+    kernels' expression, bit for bit; silu is the float64 value rounded to float32, which the kernels meet within 4
+    ulp."""
+    f = np.float32
+    v = np.asarray(v, dtype=f)
+    cshape = (1, -1) + (1,) * (v.ndim - 2)
+    with np.errstate(all="ignore"):
+        if scale is not None:
+            v = v * np.asarray(scale, dtype=f).reshape(cshape)
+        if shift is not None:
+            v = v + np.asarray(shift, dtype=f).reshape(cshape)
+        if act == "relu":
+            return np.fmax(v, f(0))
+        if act == "relu6":
+            return np.fmin(np.fmax(v, f(0)), f(6))
+        if act == "leaky_relu":
+            return np.where(v > 0, v, v * f(LEAKY_SLOPE if act_param is None else act_param))
+        if act == "hardswish":
+            return (v * np.fmin(np.fmax(v + f(3), f(0)), f(6))) / f(6)
+        if act == "silu":
+            d = v.astype(np.float64)
+            return (d / (1.0 + np.exp(-d))).astype(f)
+        assert act == "identity", act
+        return v
+
+
+def _transformed(gather, fmap, args, relu, dilation, act, act_param, in_scale, in_shift):
+    """gather(fmap, *args, relu=False, dilation=dilation) with the input transform applied to the taps inside the map;
+    the others (zero padding, invalid taps of a transposed window) stay +0."""
+    if relu:
+        raise ValueError("pass relu or act, not both")
+    X = gather(fmap, *args, relu=False, dilation=dilation)
+    ones = np.ones(fmap.shape[:1] + (1,) + fmap.shape[2:], dtype=np.float32)
+    inmap = gather(ones, *args, relu=False, dilation=dilation) != 0
+    act = "identity" if act is None else act
+    return np.where(inmap, input_transform_numpy(X, act, act_param, in_scale, in_shift), np.float32(0))
+
+
+def _xform_of(s, d):
+    """The gather's transform arguments of layer s and problem d: relu for the reference's layers, act and the
+    affine otherwise."""
+    if s.act == "relu" and not s.bn:
+        return dict(relu=True)
+    return dict(relu=None, act=s.act, act_param=s.act_param, in_scale=d.get("in_scale"), in_shift=d.get("in_shift"))
+
+
+def bn_params(c, seed):
+    """A producer BatchNorm's folded (scale, shift), float32, for a synthetic bn layer: |scale| in [0.5, 1.5] with
+    every tenth sign flipped, shift ~ N(0, 0.5) -- far enough from zero that a padded tap given the transform shows.
+    Drawn from a generator of their own, so the rest of the problem is that of the same seed without bn."""
+    r = np.random.RandomState([seed, 0xB7])
+    scale = r.uniform(0.5, 1.5, c) * np.where(r.uniform(size=c) < 0.1, -1.0, 1.0)
+    shift = 0.5 * r.standard_normal(c)
+    return scale.astype(np.float32), shift.astype(np.float32)
 
 
 def make_problem_numpy(shape: LayerShape, seed: int, noise=0.01):
     """Host (numpy) instance of a layer problem -- used by CPU tests and by the oracle leg.
     Returns dict(fmap (nbatch*B,c,H,W) f32, randx/randy (nbatch,P) i32, W2, b2, feats (N,n) f32,
-    samples (S,), X (N,c,kh,kw) f32 relu'd patches)."""
+    samples (S,), X (N,c,kh,kw) f32 relu'd patches -- the shape's input transform of them, with in_scale / in_shift
+    (bn_params) for a bn shape)."""
     if isinstance(shape, LayerShape3d):
         return _make_problem3d_numpy(shape, seed, noise)
     r = np.random.RandomState(seed)
@@ -236,22 +326,26 @@ def make_problem_numpy(shape: LayerShape, seed: int, noise=0.01):
     randy = r.randint(0, s.Wo, (s.nbatch, s.P)).astype(np.int32)
     W2 = (r.standard_normal((s.n, s.c, s.kh, s.kw)) * np.sqrt(2.0 / (s.c * s.k2))).astype(np.float32)
     b2 = (0.01 * r.standard_normal(s.n)).astype(np.float32)
-    if s.transposed:
-        X = gather_patches_tr_numpy(fmap, randx, randy, s.B, s.k, s.pad, s.stride, relu=True, dilation=s.dilation)
-    else:
-        X = gather_patches_numpy(fmap, randx, randy, s.B, s.k, s.pad, s.stride, relu=True, dilation=s.dilation)
+    bn = dict(zip(("in_scale", "in_shift"), bn_params(s.c, seed))) if s.bn else {}
+    gather = gather_patches_tr_numpy if s.transposed else gather_patches_numpy
+    X = gather(fmap, randx, randy, s.B, s.k, s.pad, s.stride, dilation=s.dilation, **_xform_of(s, bn))
     Y = X.reshape(s.N, -1).astype(np.float64) @ W2.reshape(s.n, -1).T.astype(np.float64) + b2
     Y = Y + noise * Y.std() * r.standard_normal(Y.shape)
     feats = Y.astype(np.float32)
     samples = r.randint(0, s.N, s.S)
-    return dict(fmap=fmap, randx=randx, randy=randy, W2=W2, b2=b2, feats=feats, samples=samples, X=X)
+    return dict(fmap=fmap, randx=randx, randy=randy, W2=W2, b2=b2, feats=feats, samples=samples, X=X, **bn)
 
 
-def gather_patches_numpy(fmap, randx, randy, B, k, pad, stride, relu, dilation=1):
+def gather_patches_numpy(fmap, randx, randy, B, k, pad, stride, relu, dilation=1, act=None, act_param=None,
+                         in_scale=None, in_shift=None):
     """Plain numpy statement of the patch layout (rows (batch, point, image); columns (c,kh,kw))
     used to build synthetic targets.  (The *checked* restatement of the reference's
     extract_XY lives in the oracle directory; tests compare the two.)  k, pad, stride, dilation: ints or (h, w)
-    pairs, as LayerShape takes them."""
+    pairs, as LayerShape takes them.  act, act_param, in_scale, in_shift (relu then None): the input transform of the
+    taps inside the map (input_transform_numpy), the padding +0."""
+    if act is not None or in_scale is not None or in_shift is not None:
+        return _transformed(gather_patches_numpy, fmap, (randx, randy, B, k, pad, stride), relu, dilation, act,
+                            act_param, in_scale, in_shift)
     (kh, kw), (ph, pw), (sh, sw), (dh, dw) = (conv_pair(v) for v in (k, pad, stride, dilation))
     nimg, c, H, W = fmap.shape
     nbatch, P = randx.shape
@@ -279,18 +373,24 @@ def _make_problem3d_numpy(s, seed, noise):
     randy = r.randint(0, s.Wo, (s.nbatch, s.P)).astype(np.int32)
     W2 = (r.standard_normal((s.n, s.c) + s.window) * np.sqrt(2.0 / (s.c * s.k2))).astype(np.float32)
     b2 = (0.01 * r.standard_normal(s.n)).astype(np.float32)
+    bn = dict(zip(("in_scale", "in_shift"), bn_params(s.c, seed))) if s.bn else {}
     gather = gather_patches_tr3d_numpy if s.transposed else gather_patches3d_numpy
-    X = gather(fmap, randt, randx, randy, s.B, s.k, s.pad, s.stride, relu=True, dilation=s.dilation)
+    X = gather(fmap, randt, randx, randy, s.B, s.k, s.pad, s.stride, dilation=s.dilation, **_xform_of(s, bn))
     Y = X.reshape(s.N, -1).astype(np.float64) @ W2.reshape(s.n, -1).T.astype(np.float64) + b2
     Y = Y + noise * Y.std() * r.standard_normal(Y.shape)
     feats = Y.astype(np.float32)
     samples = r.randint(0, s.N, s.S)
-    return dict(fmap=fmap, randt=randt, randx=randx, randy=randy, W2=W2, b2=b2, feats=feats, samples=samples, X=X)
+    return dict(fmap=fmap, randt=randt, randx=randx, randy=randy, W2=W2, b2=b2, feats=feats, samples=samples, X=X,
+                **bn)
 
 
-def gather_patches3d_numpy(fmap, randt, randx, randy, B, k, pad, stride, relu, dilation=1):
+def gather_patches3d_numpy(fmap, randt, randx, randy, B, k, pad, stride, relu, dilation=1, act=None, act_param=None,
+                           in_scale=None, in_shift=None):
     """gather_patches_numpy for NCDHW maps and Conv3d windows: rows (batch, point, image), columns (c, kt, kh, kw).
-    k, pad, stride, dilation: ints or (t, h, w) triples."""
+    k, pad, stride, dilation: ints or (t, h, w) triples; act ... in_shift as for gather_patches_numpy."""
+    if act is not None or in_scale is not None or in_shift is not None:
+        return _transformed(gather_patches3d_numpy, fmap, (randt, randx, randy, B, k, pad, stride), relu, dilation,
+                            act, act_param, in_scale, in_shift)
     (kt, kh, kw), (pt, ph, pw), (st, sh, sw), (dt, dh, dw) = (conv_triple(v) for v in (k, pad, stride, dilation))
     nimg, c, D, H, W = fmap.shape
     nbatch, P = randx.shape
@@ -318,10 +418,15 @@ def _tr_axis_numpy(x, pad, stride, dil, k, n):
     return np.where(ok, h, 0), ok
 
 
-def gather_patches_tr3d_numpy(fmap, randt, randx, randy, B, k, pad, stride, relu, dilation=1):
+def gather_patches_tr3d_numpy(fmap, randt, randx, randy, B, k, pad, stride, relu, dilation=1, act=None,
+                              act_param=None, in_scale=None, in_shift=None):
     """The patch gather of torch.nn.ConvTranspose3d in numpy: fmap (nimg, c, D, H, W) is the layer's input map, the
     points (t, x, y) lie in its output map; rows (batch, point, image), columns (c, kt, kh, kw), zero for invalid taps.
-    k, pad, stride, dilation: ints or (t, h, w) triples."""
+    k, pad, stride, dilation: ints or (t, h, w) triples; act ... in_shift as for gather_patches_numpy (the invalid
+    taps stay +0)."""
+    if act is not None or in_scale is not None or in_shift is not None:
+        return _transformed(gather_patches_tr3d_numpy, fmap, (randt, randx, randy, B, k, pad, stride), relu, dilation,
+                            act, act_param, in_scale, in_shift)
     (kt, kh, kw), (pt, ph, pw), (st, sh, sw), (dt, dh, dw) = (conv_triple(v) for v in (k, pad, stride, dilation))
     nimg, c, D, H, W = fmap.shape
     nbatch, P = np.asarray(randx).shape
@@ -343,9 +448,13 @@ def gather_patches_tr3d_numpy(fmap, randt, randx, randy, B, k, pad, stride, relu
     return out
 
 
-def gather_patches_tr_numpy(fmap, randx, randy, B, k, pad, stride, relu, dilation=1):
+def gather_patches_tr_numpy(fmap, randx, randy, B, k, pad, stride, relu, dilation=1, act=None, act_param=None,
+                            in_scale=None, in_shift=None):
     """gather_patches_tr3d_numpy for torch.nn.ConvTranspose2d: the one-frame case, columns (c, kh, kw).  k, pad,
-    stride, dilation: ints or (h, w) pairs."""
+    stride, dilation: ints or (h, w) pairs; act ... in_shift as for gather_patches_numpy."""
+    if act is not None or in_scale is not None or in_shift is not None:
+        return _transformed(gather_patches_tr_numpy, fmap, (randx, randy, B, k, pad, stride), relu, dilation, act,
+                            act_param, in_scale, in_shift)
     (kh, kw), (ph, pw), (sh, sw), (dh, dw) = (conv_pair(v) for v in (k, pad, stride, dilation))
     X = gather_patches_tr3d_numpy(fmap[:, :, None], np.zeros_like(randx), randx, randy, B, (1, kh, kw), (0, ph, pw),
                                   (1, sh, sw), relu, dilation=(1, dh, dw))
@@ -369,7 +478,9 @@ def make_problem_device(shape: LayerShape, seed: int, eng, noise=0.01, pinned_ho
     then carries host_layout='nhwc').
     dtype: element type of the feature maps (fmap, fmap_host): None / torch.float32, or torch.bfloat16 /
     torch.float16 as a 16-bit forward pass would hand them over -- drawn in fp32 as for float32, then rounded; the
-    targets are computed from the rounded map."""
+    targets are computed from the rounded map.
+    A bn shape's dict carries in_scale / in_shift (bn_params, fp32 on device), and its targets come from X gathered
+    through the shape's input transform."""
     import torch
 
     if isinstance(shape, LayerShape3d):
@@ -387,14 +498,15 @@ def make_problem_device(shape: LayerShape, seed: int, eng, noise=0.01, pinned_ho
     W2 = torch.randn((s.n, s.c, s.kh, s.kw), generator=g, device=dev, dtype=torch.float32) * float(
         np.sqrt(2.0 / (s.c * s.k2)))
     b2 = 0.01 * torch.randn((s.n,), generator=g, device=dev, dtype=torch.float32)
-    X = eng.patch_gather(fmap, randx, randy, s.B, s.P, relu=True, **s.conv_args())
+    bn = {nm: torch.as_tensor(v, device=dev) for nm, v in zip(("in_scale", "in_shift"), bn_params(s.c, seed))} if s.bn else {}
+    X = eng.patch_gather(fmap, randx, randy, s.B, s.P, **_xform_of(s, bn), **s.conv_args())
     Y = X.to(torch.float64) @ W2.reshape(s.n, -1).T.to(torch.float64) + b2.to(torch.float64)
     Y = Y + noise * Y.std() * torch.randn(Y.shape, generator=g, device=dev, dtype=torch.float64)
     feats = Y.to(torch.float32)
     samples = torch.as_tensor(r.randint(0, s.N, s.S).astype(np.int32), device=dev)
     seeds = r.randint(0, 2147483647, size=64)
     out = dict(fmap=fmap, randx=randx, randy=randy, W2=W2, b2=b2, feats=feats, samples=samples, seeds=seeds,
-               layout=layout)
+               layout=layout, **bn)
     del X, Y
     assert host_layout in ("nchw", "nhwc"), host_layout
     if pinned_host and host_layout == "nhwc":
@@ -430,14 +542,15 @@ def _make_problem3d_device(s, seed, eng, noise, pinned_host, layout, dtype, host
     W2 = torch.randn((s.n, s.c) + s.window, generator=g, device=dev, dtype=torch.float32) * float(
         np.sqrt(2.0 / (s.c * s.k2)))
     b2 = 0.01 * torch.randn((s.n,), generator=g, device=dev, dtype=torch.float32)
-    X = eng.patch_gather3d(fmap, *pts, s.B, s.P, relu=True, **s.conv_args())
+    bn = {nm: torch.as_tensor(v, device=dev) for nm, v in zip(("in_scale", "in_shift"), bn_params(s.c, seed))} if s.bn else {}
+    X = eng.patch_gather3d(fmap, *pts, s.B, s.P, **_xform_of(s, bn), **s.conv_args())
     Y = X.to(torch.float64) @ W2.reshape(s.n, -1).T.to(torch.float64) + b2.to(torch.float64)
     Y = Y + noise * Y.std() * torch.randn(Y.shape, generator=g, device=dev, dtype=torch.float64)
     feats = Y.to(torch.float32)
     samples = torch.as_tensor(r.randint(0, s.N, s.S).astype(np.int32), device=dev)
     seeds = r.randint(0, 2147483647, size=64)
     out = dict(fmap=fmap, randt=pts[0], randx=pts[1], randy=pts[2], W2=W2, b2=b2, feats=feats, samples=samples,
-               seeds=seeds, layout=layout, host_layout=host_layout)
+               seeds=seeds, layout=layout, host_layout=host_layout, **bn)
     del X, Y
     if pinned_host:
         src = fmap.permute(0, 2, 3, 4, 1) if host_layout == "ndhwc" else fmap

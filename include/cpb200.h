@@ -196,6 +196,42 @@ int cp_patch_gather_conv_transpose3d(cp_handle_t h, const void *fmap, int fmap_d
                                      int dil_w, int relu, float *X_out, int64_t ldx, cp_stream_t stream);
 
 /*
+ * Patch gather with the consumer's input transform: Conv-BN-activation networks pruned from their raw conv outputs.
+ * The stored map is the producer's raw output (before its BatchNorm and activation), which also serves as the
+ * producer's own Y; X of the consumer is gathered from it through the transform.  For a tap inside the map, on
+ * channel a, with v the exactly widened element:
+ *   1. with an affine: v = (v * scale[a]) + shift[a], two separately rounded fp32 operations (no FMA); in_scale or
+ *      in_shift NULL: that operation is left out.  Without either no arithmetic is done, so -0 stays -0.
+ *   2. then act, each operation rounded in fp32:
+ *        CP_ACT_IDENTITY    v
+ *        CP_ACT_RELU        fmaxf(v, 0)                       (NaN gives 0, as in the relu != 0 gathers)
+ *        CP_ACT_RELU6       fminf(fmaxf(v, 0), 6)
+ *        CP_ACT_LEAKY_RELU  v > 0 ? v : v * act_param
+ *        CP_ACT_HARDSWISH   (v * fminf(fmaxf(v + 3, 0), 6)) / 6   (PyTorch's order, IEEE division)
+ *        CP_ACT_SILU        v / (1 + expf(-v)) with the accurate expf (for v < -64, (v e) e with e = expf(v / 2),
+ *                           the same value without overflow): every path gives the same bits, within 4 ulp of the
+ *                           float64 value rounded to fp32
+ *      All but SiLU are bit for bit the NumPy float32 expression with np.fmax / np.fmin.
+ * Every tap outside the map, and every invalid tap of a transposed window, is +0.0f: the transform is not applied to
+ * it, because the consumer's zero padding pads its post-activation input (this matters as soon as shift != 0).
+ * fold_bn of an eval-mode BatchNorm: scale = weight / sqrt(running_var + eps), shift = bias - running_mean * scale.
+ *   randt  : NULL for a 2-D map (then D = 1, kt = 1, pad_t = 0, stride_t = dil_t = 1) -- the window, paths and bounds
+ *            of cp_patch_gather_conv; otherwise those of cp_patch_gather_conv3d.
+ *   transposed : != 0 for the window of nn.ConvTranspose2d / 3d (cp_patch_gather_conv_transpose / _transpose3d).
+ *   in_scale, in_shift : c fp32 values each in device memory, or NULL.
+ * Every other argument is that of the entry the window selects.  Before any device work, CP_ERR_INVALID with a message
+ * for that entry's refusals, an unknown act, a non-finite act_param, a scale or shift that does not lie in device
+ * memory, and for a 2-D call (randt NULL) a depth other than the one-frame one.  CP_ACT_RELU without an affine gives
+ * the bits of relu = 1 of the entry the window selects, CP_ACT_IDENTITY those of relu = 0.
+ */
+enum { CP_ACT_IDENTITY = 0, CP_ACT_RELU = 1, CP_ACT_RELU6 = 2, CP_ACT_LEAKY_RELU = 3, CP_ACT_HARDSWISH = 4, CP_ACT_SILU = 5 };
+int cp_patch_gather_act(cp_handle_t h, const void *fmap, int fmap_dtype, int nbatch, int B, int c, int D, int H, int W,
+                        int layout, const int32_t *randt, const int32_t *randx, const int32_t *randy, int P, int kt,
+                        int kh, int kw, int pad_t, int pad_h, int pad_w, int stride_t, int stride_h, int stride_w,
+                        int dil_t, int dil_h, int dil_w, int transposed, int act, float act_param,
+                        const float *in_scale, const float *in_shift, float *X_out, int64_t ldx, cp_stream_t stream);
+
+/*
  * Point gather -- replaces the gather of Net.extract_features (lib/net.py:509-519):
  *   Y_out[(batch*P+point)*B + image, j] = fmap[batch*B+image, j, randx, randy].
  * fp32 out (the reference widens to fp64; the bias of lib/net.py:1707 is applied
