@@ -184,7 +184,9 @@ colstat_part(const Cols C, int64_t nrows, int mtot, double *__restrict__ part, f
     }
 }
 
-// shift[o] = fl32(mean), scale[o] = 2^e with 2 * max|x| * 2^e in [2^9, 2^10), inv[o] = 2^-e (fp64)
+// shift[o] = fl32(mean), scale[o] = 2^e with 2 * max|x| * 2^e in [2^9, 2^10), inv[o] = 2^-e (fp64).
+// e comes from max|x| itself (2 max|x| overflows fp32 from 2^127 on) and is clamped to the exponents of normal fp32
+// powers of two; only columns with max|x| < 2^-119 reach the clamp, and they keep |v| < 2^10.
 __global__ void __launch_bounds__(128)
 colstat_finish(const double *__restrict__ part, const float *__restrict__ part_max, int mtot, double invN,
                float *__restrict__ shift, float *__restrict__ scale, double *__restrict__ inv) {
@@ -199,11 +201,10 @@ colstat_finish(const double *__restrict__ part, const float *__restrict__ part_m
 #pragma unroll
     for (int r = 0; r < RS; ++r) { t += v[r]; mx = fmaxf(mx, m[r]); }
     shift[o] = (float)(t * invN);
-    int e = 0;
-    const float b = 2.f * mx;  // |x - mean| <= 2 max|x|
-    if (b > 0.f && isfinite(b)) {
-        e = 9 - ilogbf(b);
-        e = e > 100 ? 100 : (e < -100 ? -100 : e);
+    int e = 0;  // |x - mean| <= 2 max|x|
+    if (mx > 0.f && isfinite(mx)) {
+        e = 8 - ilogbf(mx);
+        e = e > 127 ? 127 : (e < -126 ? -126 : e);
     }
     scale[o] = ldexpf(1.f, e);
     inv[o] = ldexp(1.0, -e);

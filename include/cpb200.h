@@ -58,7 +58,9 @@ enum {
                           accumulation per 64-row run, fp64 reduction over the runs.  The split is into two fp16
                           halves of the shifted and power-of-two scaled data (the same split precision as tf32 at
                           twice the rate; csrc/gram_tc2.cu); the name of the constant is kept for source
-                          compatibility. */
+                          compatibility.  Range: x - mean must be finite in fp32 for every column of X and of Y;
+                          inside it, scaling X or Y by a power of two that keeps their nonzero values
+                          normal fp32 scales every statistic exactly. */
 };
 
 int cp_version(void);
